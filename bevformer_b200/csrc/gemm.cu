@@ -9,10 +9,12 @@
 // (temporal_self_attention.py:198,206-209,267; spatial_cross_attention.py:173,334,338-341;
 // custom_base_transformer_layer.py:157-158).
 //
-// One kernel template serves the three products; they differ only in which operand is MN-major in shared
-// memory (the non-reduced index contiguous, i.e. the tensor read in its natural row-major layout without a
-// transpose).  Persistent CTAs of three warpgroups walk a flat list of (128 x BN output tile, reduction split)
-// units:
+// Operands differ only in which is MN-major in shared memory (the non-reduced index contiguous, i.e. the tensor
+// read in its natural row-major layout without a transpose).  Forward and dgrad run on the weight-stationary
+// kernel gemm_ws_wgmma further down (the weight tile of a column block stays in shared memory; ping-pong consumer
+// warpgroups; TMA-store epilogue).  The weight gradient, and forward / dgrad with a reduction too long for the
+// weight tile to fit (> 1024), run on gemm_bf16_wgmma: persistent CTAs of three warpgroups walking a flat list
+// of (128 x BN output tile, reduction split) units:
 //   warpgroup 0, warp 0   TMA producer: cp.async.bulk.tensor loads of the A (128 x 64) and B (BN x 64) k-blocks
 //                          into a ring of SWIZZLE_128B shared-memory stages, completion on mbarriers
 //   warpgroup 0, warp 1   weight gradient only: column sums of the dY tiles straight from the same stages (db)
@@ -22,8 +24,7 @@
 //                          i.e. the loads of tile i+1 overlap the epilogue of tile i.
 //   epilogue               straight from the accumulator registers: bias, ReLU, addend, convert, store (or fp32
 //                          reduction / per-split slab for the weight gradient).
-// These GEMMs have K = 256 or 512 only: they are bound by streaming X / Y through HBM; the weight tile of a
-// column block (<= 64 KB) stays hot in the 50 MB L2 across the row tiles that reuse it.
+// These GEMMs have K = 256 or 512 only: they are bound by streaming X / Y through HBM.
 #include <cuda.h>
 
 #include <cstdlib>
@@ -129,6 +130,38 @@ template <int kTA, int kTB> struct Wgmma<128, kTA, kTB> {
                      "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]),
                      "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]),
                      "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+                     : "l"(da), "l"(db), "r"((int)accumulate), "n"(kTA), "n"(kTB));
+    }
+};
+template <int kTA, int kTB> struct Wgmma<256, kTA, kTB> {
+    __device__ static __forceinline__ void run(float (&d)[128], uint64_t da, uint64_t db, bool accumulate) {
+        asm volatile("{\n.reg .pred p;\nsetp.ne.b32 p, %130, 0;\n"
+                     "wgmma.mma_async.sync.aligned.m64n256k16.f32.bf16.bf16 {"
+                     "%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
+                     "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, "
+                     "%32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, "
+                     "%48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63, "
+                     "%64, %65, %66, %67, %68, %69, %70, %71, %72, %73, %74, %75, %76, %77, %78, %79, "
+                     "%80, %81, %82, %83, %84, %85, %86, %87, %88, %89, %90, %91, %92, %93, %94, %95, "
+                     "%96, %97, %98, %99, %100, %101, %102, %103, %104, %105, %106, %107, %108, %109, %110, %111, "
+                     "%112, %113, %114, %115, %116, %117, %118, %119, %120, %121, %122, %123, %124, %125, %126, %127"
+                     "}, %128, %129, p, 1, 1, %131, %132;\n}\n"
+                     : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
+                     "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]),
+                     "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]),
+                     "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]),
+                     "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]),
+                     "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]),
+                     "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]),
+                     "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63]),
+                     "+f"(d[64]), "+f"(d[65]), "+f"(d[66]), "+f"(d[67]), "+f"(d[68]), "+f"(d[69]), "+f"(d[70]), "+f"(d[71]),
+                     "+f"(d[72]), "+f"(d[73]), "+f"(d[74]), "+f"(d[75]), "+f"(d[76]), "+f"(d[77]), "+f"(d[78]), "+f"(d[79]),
+                     "+f"(d[80]), "+f"(d[81]), "+f"(d[82]), "+f"(d[83]), "+f"(d[84]), "+f"(d[85]), "+f"(d[86]), "+f"(d[87]),
+                     "+f"(d[88]), "+f"(d[89]), "+f"(d[90]), "+f"(d[91]), "+f"(d[92]), "+f"(d[93]), "+f"(d[94]), "+f"(d[95]),
+                     "+f"(d[96]), "+f"(d[97]), "+f"(d[98]), "+f"(d[99]), "+f"(d[100]), "+f"(d[101]), "+f"(d[102]), "+f"(d[103]),
+                     "+f"(d[104]), "+f"(d[105]), "+f"(d[106]), "+f"(d[107]), "+f"(d[108]), "+f"(d[109]), "+f"(d[110]), "+f"(d[111]),
+                     "+f"(d[112]), "+f"(d[113]), "+f"(d[114]), "+f"(d[115]), "+f"(d[116]), "+f"(d[117]), "+f"(d[118]), "+f"(d[119]),
+                     "+f"(d[120]), "+f"(d[121]), "+f"(d[122]), "+f"(d[123]), "+f"(d[124]), "+f"(d[125]), "+f"(d[126]), "+f"(d[127])
                      : "l"(da), "l"(db), "r"((int)accumulate), "n"(kTA), "n"(kTB));
     }
 };
@@ -350,6 +383,236 @@ gemm_bf16_wgmma(const __grid_constant__ CUtensorMap map_a, const __grid_constant
     }
 }
 
+// ================================================================================================
+// Weight-stationary forward / dgrad:  Y[M, N] = act( A[M, R] . B + bias ) (+ addend),  A K-major,
+// B = the weight, K-major (forward, W[N, R]) or MN-major (dgrad, W[R, N] read in place).
+//
+// CTA b owns column block b % tiles_n for its whole life and a contiguous range of 64-row tiles; the CTAs
+// of one column block split the rows evenly, and CTA g * tiles_n + j (j = 0 .. tiles_n - 1) walk the same
+// rows in step, so an activation row read from HBM by one column block is an L2 hit for the others.
+//   warp 0 / warp 1 (lane 0)  TMA producers of consumer warpgroup 1 / 2: the BN x R weight tile once (warp 0),
+//                             then the 64 x 64 A k-blocks of that warpgroup's tiles through its own ring, and
+//                             the tile's addend (bf16, 64 x BN) into its staging buffer
+//   warpgroups 1 and 2        ping-pong: each owns every other row tile of the range whole (m64nBNk16 wgmmas
+//                             against the resident weight, one group in flight behind the one being issued),
+//                             so one warpgroup's epilogue runs while the other issues its wgmmas
+//   epilogue                  bias, ReLU, addend (from the staging buffer) in registers, convert, write into
+//                             the SWIZZLE_128B staging buffer, cp.async.bulk.tensor store; rows past M and
+//                             columns past N are clipped by the tensor map
+// Shared memory (227 KB): weight BN x R x 2 (<= 128 KB) + 2 x staging (64 rows x min(BN x out bytes, 512 B))
+// + 2 x ring (stages x 8 KB), the ring taking what is left (at most kMaxStages):
+//   BN 256, R 256: 128 + 2 x 32 + 2 x 2 x 8 KB     BN 128, R 512: 128 + 2 x 16 (bf16) / 32 (fp32) + 2 x 4 / 2 x 8 KB
+//   BN 256, R 192:  96 + 2 x 32 + 2 x 4 x 8 KB     BN  64, R 768:  96 + 2 x 8 + 2 x 6 x 8 KB
+// ================================================================================================
+constexpr int kWsRows = 64;               // rows per tile: one consumer warpgroup, m64
+constexpr int kWsBoxBytes = 64 * 128;     // one 64-row x 128 B TMA box (A k-block, addend/output box)
+constexpr int kWsStageMax = 4 * kWsBoxBytes;
+constexpr int kWsWeightMax = 128 * 1024;
+
+struct WsParams {
+    int M, N, R;           // output rows / columns, reduction length (multiple of 64)
+    int tiles_m, tiles_n, groups;
+    int stages;            // A ring depth per consumer warpgroup
+    int stg_bytes;         // staging buffer per consumer warpgroup
+    int relu;
+    const void *bias;      // (N) f32 or bf16, or null
+    int bias_bf16;
+    int addend;            // 1: (M, N) bf16 addend (map_add) added after the activation
+    int out_f32;
+};
+
+__device__ __forceinline__ void tma_store_2d(const CUtensorMap *map, const void *src, int c0, int c1) {
+    asm volatile("cp.async.bulk.tensor.2d.global.shared::cta.bulk_group [%0, {%2, %3}], [%1];"
+                 ::"l"(map), "r"(smem_u32(src)), "r"(c0), "r"(c1) : "memory");
+}
+
+template <int BN, bool kBmn>
+__global__ void __launch_bounds__(kGemmThreads, 1)
+gemm_ws_wgmma(const __grid_constant__ CUtensorMap map_a, const __grid_constant__ CUtensorMap map_w,
+              const __grid_constant__ CUtensorMap map_y, const __grid_constant__ CUtensorMap map_add,
+              const WsParams p) {
+    static_assert(BN == 64 || BN == 128 || BN == 256, "tile width");
+    extern __shared__ __align__(1024) uint8_t smem_raw[];
+    uint8_t *smem = reinterpret_cast<uint8_t *>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
+    const int kblocks = p.R / kBK;
+    const int w_bytes = kblocks * BN * 128;
+    uint8_t *sw = smem;
+    uint8_t *stg0 = sw + w_bytes;
+    uint8_t *ring0 = stg0 + 2 * p.stg_bytes;
+    uint64_t *bars = reinterpret_cast<uint64_t *>(ring0 + 2 * p.stages * kWsBoxBytes);
+    uint64_t *w_full = bars;
+    uint64_t *full = bars + 1, *empty = full + 2 * kMaxStages;          // [warpgroup][stage]
+    uint64_t *add_full = empty + 2 * kMaxStages, *stg_empty = add_full + 2;
+    float *sbias = reinterpret_cast<float *>(stg_empty + 2);
+
+    const int wg = threadIdx.x >> 7, warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    const int tn = blockIdx.x % p.tiles_n, g = blockIdx.x / p.tiles_n;
+    const int t_begin = (int)((int64_t)g * p.tiles_m / p.groups);
+    const int t_end = (int)((int64_t)(g + 1) * p.tiles_m / p.groups);
+    const int col0 = tn * BN;
+
+    if (threadIdx.x == 0) {
+        asm volatile("prefetch.tensormap [%0];" ::"l"(&map_a) : "memory");
+        asm volatile("prefetch.tensormap [%0];" ::"l"(&map_w) : "memory");
+        asm volatile("prefetch.tensormap [%0];" ::"l"(&map_y) : "memory");
+        mbar_init(w_full, 1);
+        for (int i = 0; i < 2 * kMaxStages; ++i) { mbar_init(&full[i], 1); mbar_init(&empty[i], 4); }
+        for (int i = 0; i < 2; ++i) { mbar_init(&add_full[i], 1); mbar_init(&stg_empty[i], 1); }
+        asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+    }
+    __syncthreads();
+
+    if (wg == 0) {
+        asm volatile("setmaxnreg.dec.sync.aligned.u32 40;\n" ::: "memory");
+        // ===================== TMA producers: warp c feeds consumer warpgroup c ==================
+        if (warp < 2 && lane == 0) {
+            const int c = warp;
+            if (c == 0) {
+                // columns of the block past N are not loaded (MN-major) or read as zeros (K-major); either way
+                // they only reach output columns the store clips
+                const int chunks = kBmn ? min(BN / 64, (p.N - col0 + 63) / 64) : 1;
+                mbar_expect_tx(w_full, (uint32_t)(kblocks * (kBmn ? chunks * kChunk : BN * 128)));
+                for (int kb = 0; kb < kblocks; ++kb) {
+                    uint8_t *dst = sw + (size_t)kb * BN * 128;
+                    if (!kBmn) {
+                        tma_load_2d(dst, &map_w, w_full, kb * kBK, col0);
+                    } else {
+                        for (int ch = 0; ch < chunks; ++ch)
+                            tma_load_2d(dst + ch * kChunk, &map_w, w_full, col0 + ch * 64, kb * kBK);
+                    }
+                }
+            }
+            uint8_t *ring = ring0 + (size_t)c * p.stages * kWsBoxBytes, *stg = stg0 + (size_t)c * p.stg_bytes;
+            uint64_t *f = full + c * kMaxStages, *e = empty + c * kMaxStages;
+            const int add_boxes = min(BN / 64, (p.N - col0 + 63) / 64);
+            int s = 0; uint32_t ph = 0, t = 0;
+            for (int tm = t_begin + c; tm < t_end; tm += 2, ++t) {
+                for (int kb = 0; kb < kblocks; ++kb) {
+                    mbar_wait(&e[s], ph ^ 1);
+                    mbar_expect_tx(&f[s], (uint32_t)kWsBoxBytes);
+                    tma_load_2d(ring + (size_t)s * kWsBoxBytes, &map_a, &f[s], kb * kBK, tm * kWsRows);
+                    if (++s == p.stages) { s = 0; ph ^= 1; }
+                }
+                if (p.addend) {
+                    if (t > 0) mbar_wait(&stg_empty[c], (t - 1) & 1);
+                    mbar_expect_tx(&add_full[c], (uint32_t)(add_boxes * kWsBoxBytes));
+                    for (int b = 0; b < add_boxes; ++b)
+                        tma_load_2d(stg + b * kWsBoxBytes, &map_add, &add_full[c], col0 + b * 64, tm * kWsRows);
+                }
+            }
+        }
+        return;
+    }
+    asm volatile("setmaxnreg.inc.sync.aligned.u32 232;\n" ::: "memory");
+
+    // ===================== consumers: warpgroup cw owns row tiles t_begin + cw, t_begin + cw + 2, ... =========
+    const int cw = wg - 1, w4 = warp & 3;
+    const bool leader = (threadIdx.x & 127) == 0;
+    uint8_t *ring = ring0 + (size_t)cw * p.stages * kWsBoxBytes, *stg = stg0 + (size_t)cw * p.stg_bytes;
+    uint64_t *f = full + cw * kMaxStages, *e = empty + cw * kMaxStages;
+    // fp32 output of a 256-wide block goes out in two staging fills of 128 columns
+    constexpr int kF32PassCols = BN > 128 ? 128 : BN;
+    const int passes = p.out_f32 ? BN / kF32PassCols : 1;
+    const uint32_t sw_base = smem_u32(sw);
+    constexpr uint64_t db_step = kBmn ? 128 : 2;
+    float acc[BN / 2];
+    // the block's bias as fp32 (zeros past N or without a bias), read from shared memory by the epilogue
+    for (int i = threadIdx.x - 128; i < BN; i += 256) {
+        const int col = col0 + i;
+        float b = 0.f;
+        if (p.bias && col < p.N)
+            b = p.bias_bf16 ? __bfloat162float(reinterpret_cast<const bf16 *>(p.bias)[col])
+                            : reinterpret_cast<const float *>(p.bias)[col];
+        sbias[i] = b;
+    }
+    asm volatile("bar.sync 3, 256;" ::: "memory");
+    mbar_wait(w_full, 0);
+    int s = 0; uint32_t ph = 0, t = 0;
+    for (int tm = t_begin + cw; tm < t_end; tm += 2, ++t) {
+        int prev = -1;
+        for (int kb = 0; kb < kblocks; ++kb) {
+            mbar_wait(&f[s], ph);
+            const uint64_t da = smem_desc_sw128(smem_u32(ring + (size_t)s * kWsBoxBytes), 0);
+            const uint64_t db = smem_desc_sw128(sw_base + (uint32_t)(kb * BN * 128), kChunk);
+            wgmma_fence();
+#pragma unroll
+            for (int k = 0; k < kBK / 16; ++k)
+                Wgmma<BN, 0, kBmn>::run(acc, da + 2 * k, db + db_step * k, (kb | k) != 0);
+            wgmma_commit();
+            if (prev >= 0) {
+                // the group of k-block kb - 1 has retired: its A stage can be refilled
+                asm volatile("wgmma.wait_group.sync.aligned 1;" ::: "memory");
+                __syncwarp();
+                if (lane == 0) mbar_arrive(&e[prev]);
+            }
+            prev = s;
+            if (++s == p.stages) { s = 0; ph ^= 1; }
+        }
+        wgmma_wait0();
+        fence_regs(acc);
+        __syncwarp();
+        if (lane == 0) mbar_arrive(&e[prev]);
+
+        // ---- epilogue: thread holds rows r0 (h = 0) and r0 + 8 (h = 1), columns 8 j + cq, 8 j + cq + 1
+        const int r0 = w4 * 16 + (lane >> 2), cq = 2 * (lane & 3);
+        if (p.addend) mbar_wait(&add_full[cw], t & 1);
+#pragma unroll
+        for (int j = 0; j < BN / 8; ++j) {
+            const float2 bv = *reinterpret_cast<const float2 *>(sbias + 8 * j + cq);
+            const float b0 = bv.x, b1 = bv.y;
+#pragma unroll
+            for (int h = 0; h < 2; ++h) {
+                float v0 = acc[4 * j + 2 * h] + b0, v1 = acc[4 * j + 2 * h + 1] + b1;
+                if (p.relu) { v0 = fmaxf(v0, 0.f); v1 = fmaxf(v1, 0.f); }
+                if (p.addend) {
+                    // bf16 box j / 8, 16 B unit j % 8 of row r, stored at unit (j % 8) ^ (r % 8)
+                    const int r = r0 + 8 * h;
+                    const uint32_t a2 = *reinterpret_cast<const uint32_t *>(
+                        stg + (j >> 3) * kWsBoxBytes + r * 128 + (((j & 7) ^ (r & 7)) << 4) + 2 * cq);
+                    v0 += bf16_lo(a2); v1 += bf16_hi(a2);
+                }
+                acc[4 * j + 2 * h] = v0; acc[4 * j + 2 * h + 1] = v1;
+            }
+        }
+#pragma unroll
+        for (int pass = 0; pass < 2; ++pass) {
+            if (pass == passes) break;
+            // the previous store has finished reading the staging buffer (leader waited) and the addend is read
+            asm volatile("bar.sync %0, 128;" ::"r"(1 + cw) : "memory");
+#pragma unroll
+            for (int j = 0; j < BN / 8; ++j) {
+#pragma unroll
+                for (int h = 0; h < 2; ++h) {
+                    const int r = r0 + 8 * h;
+                    const float v0 = acc[4 * j + 2 * h], v1 = acc[4 * j + 2 * h + 1];
+                    if (p.out_f32) {
+                        // fp32 box jj / 4 of this pass, 16 B unit 2 (jj % 4) + cq / 4
+                        if (j * 8 / kF32PassCols != pass) continue;
+                        const int jj = j - pass * (kF32PassCols / 8);
+                        const int unit = 2 * (jj & 3) + (cq >> 2);
+                        *reinterpret_cast<float2 *>(stg + (jj >> 2) * kWsBoxBytes + r * 128 + ((unit ^ (r & 7)) << 4) +
+                                                    4 * (cq & 3)) = make_float2(v0, v1);
+                    } else {
+                        *reinterpret_cast<uint32_t *>(stg + (j >> 3) * kWsBoxBytes + r * 128 +
+                                                      (((j & 7) ^ (r & 7)) << 4) + 2 * cq) = pack_bf16x2(v0, v1);
+                    }
+                }
+            }
+            asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
+            asm volatile("bar.sync %0, 128;" ::"r"(1 + cw) : "memory");
+            if (leader) {
+                const int cols_per_box = p.out_f32 ? 32 : 64, pc0 = col0 + pass * (BN / passes);
+                for (int b = 0; b < BN / passes / cols_per_box && pc0 + b * cols_per_box < p.N; ++b)
+                    tma_store_2d(&map_y, stg + b * kWsBoxBytes, pc0 + b * cols_per_box, tm * kWsRows);
+                asm volatile("cp.async.bulk.commit_group;" ::: "memory");
+                asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory");
+            }
+        }
+        if (leader && p.addend) mbar_arrive(&stg_empty[cw]);
+    }
+    if (leader) asm volatile("cp.async.bulk.wait_group 0;" ::: "memory");
+}
+
 // second pass of the two-pass weight gradient: dW[n, k] = sum over splits of the partial slabs, written
 // in the parameter's own dtype (no zero-fill, no cast kernel); db likewise.
 template <typename TO>
@@ -401,16 +664,19 @@ static EncodeTiledFn encode_tiled_fn() {
     return fn;
 }
 
-// row-major (rows, cols) bf16; box = box_rows x 64 elements (128 B inner), SWIZZLE_128B; out-of-range rows and
-// columns of a box read as zeros (and still count towards the transaction bytes)
-static int make_map_2d(CUtensorMap *map, const void *ptr, uint64_t rows, uint64_t cols, uint32_t box_rows) {
+// row-major (rows, cols) bf16 (or fp32); box = box_rows x 128 B, SWIZZLE_128B; out-of-range rows and columns of a
+// box read as zeros (and still count towards the transaction bytes), and are not written by a store
+static int make_map_2d(CUtensorMap *map, const void *ptr, uint64_t rows, uint64_t cols, uint32_t box_rows,
+                       bool f32 = false) {
     EncodeTiledFn encode = encode_tiled_fn();
     if (!encode) return -1;
+    const uint32_t esz = f32 ? 4 : 2;
     cuuint64_t dims[2] = {cols, rows};
-    cuuint64_t strides[1] = {cols * sizeof(uint16_t)};
-    cuuint32_t box[2] = {64, box_rows};
+    cuuint64_t strides[1] = {cols * esz};
+    cuuint32_t box[2] = {128 / esz, box_rows};
     cuuint32_t estr[2] = {1, 1};
-    CUresult r = encode(map, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, const_cast<void *>(ptr), dims,
+    CUresult r = encode(map, f32 ? CU_TENSOR_MAP_DATA_TYPE_FLOAT32 : CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2,
+                        const_cast<void *>(ptr), dims,
                         strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
                         CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
                         CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
@@ -440,6 +706,78 @@ static int launch_gemm(const char *who, const CUtensorMap &map_a, const CUtensor
     const int grid = units < device_sms() ? units : device_sms();
     gemm_bf16_wgmma<BN, kAmn, kBmn><<<grid, kGemmThreads, smem, st>>>(map_a, map_b, p);
     return check_launch(who);
+}
+
+// Column block of the weight-stationary kernel: the widest of 256 / 128 / 64 whose BN x R weight tile fits in
+// kWsWeightMax and that the N output columns do not leave more than half empty; 0 if not even 64 fits
+// (reductions longer than 1024, which the encoder never runs, go to the streamed kernel above).
+static int ws_block(int N, int R) {
+    int bn = 256;
+    while (bn > 64 && (bn * R * 2 > kWsWeightMax || bn / 2 >= N)) bn /= 2;
+    return bn * R * 2 <= kWsWeightMax ? bn : 0;
+}
+
+template <int BN, bool kBmn>
+static int launch_ws(const char *who, const CUtensorMap &map_a, const CUtensorMap &map_w, const CUtensorMap &map_y,
+                     const CUtensorMap &map_add, WsParams p, cudaStream_t st) {
+    constexpr int kSmemMax = 227 * 1024;
+    constexpr int kBarBytes = (1 + 4 * kMaxStages + 4) * 8 + BN * 4;   // + the bias block
+    p.stg_bytes = kWsRows * BN * (p.out_f32 ? 4 : 2);
+    if (p.stg_bytes > kWsStageMax) p.stg_bytes = kWsStageMax;
+    const int w_bytes = p.R * BN * 2;
+    int stages = (kSmemMax - 1024 - kBarBytes - w_bytes - 2 * p.stg_bytes) / (2 * kWsBoxBytes);
+    if (stages > kMaxStages) stages = kMaxStages;
+    if (stages < 2) return fail("%s: no room for a two-stage A ring next to the weight tile", who);
+    p.stages = stages;
+    const size_t smem = 1024 + (size_t)w_bytes + 2 * p.stg_bytes + 2 * (size_t)stages * kWsBoxBytes + kBarBytes;
+    static bool configured = false;
+    if (!configured) {
+        if (cudaFuncSetAttribute(gemm_ws_wgmma<BN, kBmn>, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmemMax) !=
+            cudaSuccess) {
+            cudaGetLastError();
+            return fail("%s: cannot reserve shared memory for the GEMM", who);
+        }
+        configured = true;
+    }
+    p.tiles_m = (p.M + kWsRows - 1) / kWsRows;
+    p.tiles_n = (p.N + BN - 1) / BN;
+    p.groups = device_sms() / p.tiles_n;
+    if (p.groups > p.tiles_m) p.groups = p.tiles_m;
+    if (p.groups < 1) p.groups = 1;
+    gemm_ws_wgmma<BN, kBmn><<<p.groups * p.tiles_n, kGemmThreads, smem, st>>>(map_a, map_w, map_y, map_add, p);
+    return check_launch(who);
+}
+
+// Y (M, N) = act(A (M, R) . B + bias) (+ addend) on the weight-stationary kernel; B is W (N, R) for the forward
+// product, or W (R, N) read in place (MN-major) for the input gradient.
+static int linear_ws(const char *who, int bn, bool b_mn, const void *a, const void *w, const void *bias, int bias_bf16,
+                     const void *addend, void *y, bool out_f32, int M, int N, int R, int relu, cudaStream_t st) {
+    CUtensorMap map_a, map_w, map_y, map_add;
+    if (int e = make_map_2d(&map_a, a, (uint64_t)M, (uint64_t)R, kWsRows))
+        return fail("%s: cuTensorMapEncodeTiled(A) failed (%lld)", who, e);
+    if (int e = b_mn ? make_map_2d(&map_w, w, (uint64_t)R, (uint64_t)N, 64)
+                     : make_map_2d(&map_w, w, (uint64_t)N, (uint64_t)R, (uint32_t)bn))
+        return fail("%s: cuTensorMapEncodeTiled(B) failed (%lld)", who, e);
+    if (int e = make_map_2d(&map_y, y, (uint64_t)M, (uint64_t)N, kWsRows, out_f32))
+        return fail("%s: cuTensorMapEncodeTiled(Y) failed (%lld)", who, e);
+    map_add = map_y;
+    if (addend)
+        if (int e = make_map_2d(&map_add, addend, (uint64_t)M, (uint64_t)N, kWsRows))
+            return fail("%s: cuTensorMapEncodeTiled(addend) failed (%lld)", who, e);
+    WsParams p;
+    memset(&p, 0, sizeof(p));
+    p.M = M; p.N = N; p.R = R;
+    p.relu = relu; p.bias = bias; p.bias_bf16 = bias_bf16;
+    p.addend = addend != nullptr; p.out_f32 = out_f32;
+    switch (bn * 2 + (int)b_mn) {
+        case 512: return launch_ws<256, false>(who, map_a, map_w, map_y, map_add, p, st);
+        case 513: return launch_ws<256, true>(who, map_a, map_w, map_y, map_add, p, st);
+        case 256: return launch_ws<128, false>(who, map_a, map_w, map_y, map_add, p, st);
+        case 257: return launch_ws<128, true>(who, map_a, map_w, map_y, map_add, p, st);
+        case 128: return launch_ws<64, false>(who, map_a, map_w, map_y, map_add, p, st);
+        case 129: return launch_ws<64, true>(who, map_a, map_w, map_y, map_add, p, st);
+    }
+    return fail("%s: no weight-stationary tile for this shape", who);
 }
 
 static GemmParams base_params(int M, int N, int R) {
@@ -476,6 +814,9 @@ static int linear_dgrad_impl(const char *who, const void *dy, const void *w, con
     if (M >= (1ll << 31)) return fail("%s: M too large", who);
     if (!aligned16(dy) || !aligned16(w) || !aligned16(dx)) return fail("%s: pointers must be 16-byte aligned", who);
     // dX (M, K) = dY (M, N) . W (N, K): A = dY K-major, B = W with its output columns contiguous (MN-major)
+    cudaStream_t st = (cudaStream_t)stream;
+    if (int bn = ws_block(K, N))
+        return linear_ws(who, bn, true, dy, w, nullptr, 0, addend, dx, false, (int)M, K, N, 0, st);
     CUtensorMap map_a, map_b;
     if (int e = make_map_2d(&map_a, dy, (uint64_t)M, (uint64_t)N, kBM))
         return fail("%s: cuTensorMapEncodeTiled(A) failed (%lld)", who, e);
@@ -484,7 +825,6 @@ static int linear_dgrad_impl(const char *who, const void *dy, const void *w, con
     GemmParams p = base_params((int)M, K, N);
     p.addend = reinterpret_cast<const bf16 *>(addend);
     p.y = dx;
-    cudaStream_t st = (cudaStream_t)stream;
     return K % 128 == 0 ? launch_gemm<128, false, true>(who, map_a, map_b, p, st)
                         : launch_gemm<64, false, true>(who, map_a, map_b, p, st);
 }
@@ -505,6 +845,10 @@ extern "C" int bevf_linear_forward(const void *x, const void *w, const void *bia
     if (y_dtype != BEVF_DTYPE_BF16 && y_dtype != BEVF_DTYPE_F32) return fail("%s: unsupported dtype code", who);
     if (bias && bias_dtype != BEVF_DTYPE_BF16 && bias_dtype != BEVF_DTYPE_F32)
         return fail("%s: unsupported bias dtype code", who);
+    cudaStream_t st = (cudaStream_t)stream;
+    if (int bn = ws_block(N, K))
+        return linear_ws(who, bn, false, x, w, bias, bias_dtype == BEVF_DTYPE_BF16, residual, y,
+                         y_dtype == BEVF_DTYPE_F32, (int)M, N, K, relu, st);
     // a column tile of 128 unless N is small (a partial last tile is clipped in the epilogue)
     const bool wide = N > 64;
     CUtensorMap map_a, map_b;
@@ -516,7 +860,6 @@ extern "C" int bevf_linear_forward(const void *x, const void *w, const void *bia
     p.relu = relu; p.bias = bias; p.bias_bf16 = bias_dtype == BEVF_DTYPE_BF16;
     p.addend = reinterpret_cast<const bf16 *>(residual);
     p.y = y; p.out_f32 = y_dtype == BEVF_DTYPE_F32;
-    cudaStream_t st = (cudaStream_t)stream;
     return wide ? launch_gemm<128, false, false>(who, map_a, map_b, p, st)
                 : launch_gemm<64, false, false>(who, map_a, map_b, p, st);
 }

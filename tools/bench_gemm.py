@@ -41,7 +41,7 @@ def main():
     args = ap.parse_args()
     dev = "cuda"
     flush = torch.empty(256 << 20, dtype=torch.uint8, device=dev)
-    hbm = 6571.2
+    hbm = 3350.0  # H100 SXM data sheet, GB/s
     try:
         hbm = json.load(open(os.path.join(os.path.dirname(__file__), "..", "MEASURED_PEAKS.json")))["hbm_gbs"]
     except Exception:
