@@ -43,6 +43,13 @@ SIGNATURES = {
                                               c_int, c_void_p, c_void_p, c_void_p, c_int, c_void_p, c_void_p, c_void_p,
                                               c_void_p] + [c_int] * 7 + [c_void_p]),
     "bevf_gv_merge": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_void_p]),
+    "bevf_msda_fx_frac_bits": (c_int, [c_int64, c_int, c_int]),
+    "bevf_msda_backward_fx": (c_int, [c_void_p, c_int, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int,
+                                      c_void_p, c_void_p, c_int, c_void_p, c_void_p] + [c_int] * 7 + [c_void_p]),
+    "bevf_msda_rows_backward_fx": (c_int, [c_void_p, c_int, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int,
+                                           c_void_p, c_void_p, c_int, c_void_p, c_void_p, c_void_p] + [c_int] * 7
+                                   + [c_void_p]),
+    "bevf_msda_fx_convert": (c_int, [c_void_p, c_void_p, c_int, c_void_p, c_int, c_int, c_int64, c_void_p]),
     "bevf_msda_rows_backward_dense": (c_int, [c_void_p, c_int, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p,
                                               c_void_p, c_int, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p]
                                       + [c_int] * 7 + [c_void_p]),
@@ -64,6 +71,11 @@ SIGNATURES = {
                                 + [c_void_p] * 4
                                 + [c_int64, c_int, ctypes.c_float, ctypes.c_uint64, c_void_p, c_int,
                                    c_void_p]),
+    "bevf_layernorm_backward_workspace_bytes": (c_int64, [c_int64, c_int]),
+    "bevf_layernorm_backward_det": (c_int, [c_void_p] * 3 + [c_int] + [c_void_p] * 4 + [c_int64]
+                                    + [c_void_p] * 5 + [c_int64]
+                                    + [c_int64, c_int, ctypes.c_float, ctypes.c_uint64, c_void_p, c_int,
+                                       c_void_p]),
     "bevf_sca_combine_forward": (c_int, [c_void_p] * 4 + [c_int] * 6 + [c_void_p]),
     "bevf_sca_combine_backward": (c_int, [c_void_p] * 4 + [c_int] * 5 + [c_void_p]),
     "bevf_linear_forward": (c_int, [c_void_p] * 3 + [c_int] + [c_void_p] * 2
@@ -76,7 +88,10 @@ SIGNATURES = {
     "bevf_linear_wgrad_out": (c_int, [c_void_p] * 4 + [c_int, c_void_p, c_int64, c_int64, c_int, c_int,
                                                       c_void_p]),
     "bevf_sum_tensors": (c_int, [c_void_p, c_int, c_void_p, c_int64, c_int, c_void_p]),
+    "bevf_linear_wgrad_into": (c_int, [c_void_p] * 5 + [c_int64, c_int64, c_int, c_int, c_void_p]),
     "bevf_colsum": (c_int, [c_void_p, c_void_p, c_int64, c_int, c_int, c_void_p]),
+    "bevf_colsum_workspace_bytes": (c_int64, [c_int64, c_int]),
+    "bevf_colsum_det": (c_int, [c_void_p, c_void_p, c_void_p, c_int64, c_int64, c_int, c_int, c_void_p]),
     "bevf_dropout_inplace": (c_int, [c_void_p, c_int64, ctypes.c_float, ctypes.c_uint64, c_void_p, c_int,
                                      c_void_p]),
     "bevf_relu_dropout_backward": (c_int, [c_void_p, c_void_p, c_void_p, c_int64, ctypes.c_float, c_int,

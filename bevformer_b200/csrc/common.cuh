@@ -165,4 +165,26 @@ __device__ __forceinline__ float gv16_scale(unsigned amax_bits) {
     return __uint_as_float((unsigned)ex << 23);                    // 2^(3 - e)
 }
 
+// ---- grad_value summed in 64-bit FIXED POINT (deterministic mode; msda.cu, gvfx.cu) --------------------------------
+// Integer addition is associative, so red.global.add.u64 of two's-complement values gives the same bits in any order.
+// bounds[0] / bounds[1] hold the bits of max|attn| / max|grad_out| with the sign cleared: as unsigned numbers NaN >
+// inf > every finite value, so a non-finite input shows in the maximum.  Every contribution w * attn * g (w <= 1) is
+// below 2^fx_exponent(bounds) and is stored as round(contribution * 2^(frac_bits - fx_exponent)).
+__host__ __device__ __forceinline__ bool fx_bounds_finite(unsigned a_bits, unsigned g_bits) {
+    return a_bits < 0x7f800000u && g_bits < 0x7f800000u;
+}
+__host__ __device__ __forceinline__ int fx_exponent(unsigned a_bits, unsigned g_bits) {
+    // a value with biased exponent field f (f = 0: zero or denormal) is below 2^(max(f, 1) - 126)
+    const int ea = (int)(a_bits >> 23 > 1u ? a_bits >> 23 : 1u) - 126;
+    const int eg = (int)(g_bits >> 23 > 1u ? g_bits >> 23 : 1u) - 126;
+    return ea + eg;
+}
+// 2^e as a double, -1022 <= e <= 1023
+__device__ __forceinline__ double fx_pow2(int e) { return __longlong_as_double((long long)(1023 + e) << 52); }
+// one contribution q * g (exact in double: two fp32 factors) scaled by a power of two and rounded to nearest
+__device__ __forceinline__ void red_add_fx(long long *p, float q, float g, double scale) {
+    const long long v = __double2ll_rn((double)q * (double)g * scale);
+    asm volatile("red.global.add.u64 [%0], %1;" :: "l"(p), "l"(v) : "memory");
+}
+
 }  // namespace bevf

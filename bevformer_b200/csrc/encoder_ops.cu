@@ -297,10 +297,12 @@ sca_prep_bwd_m8(const float *__restrict__ raw, const float *__restrict__ grad_lo
 // column sums of a (rows, C) matrix into fp32 (bias gradients): out[c] += sum_r x[r, c]
 // thread -> (column vector cv, row lane rl); consecutive threads walk along a row (coalesced 16 B
 // loads), four rows in flight per thread; row lanes are combined through shared memory without
-// atomics, then one global atomicAdd per column per CTA.
+// atomics, then one global atomicAdd per column per CTA -- or, with `part` (deterministic mode), the CTA's row of
+// column sums stored into part[blockIdx.x] for partials_add_kernel.
 template <typename T>
 __global__ void __launch_bounds__(kEThreads)
-colsum_kernel(const T *__restrict__ x, float *__restrict__ out, long long rows, int C, int rows_per_cta) {
+colsum_kernel(const T *__restrict__ x, float *__restrict__ out, long long rows, int C, int rows_per_cta,
+              float *__restrict__ part = nullptr) {
     constexpr int VEC = (sizeof(T) == 2) ? 8 : 4;
     const int per_row = C / VEC;
     const int cv = threadIdx.x % per_row, rl = threadIdx.x / per_row, rstep = kEThreads / per_row;
@@ -336,7 +338,8 @@ colsum_kernel(const T *__restrict__ x, float *__restrict__ out, long long rows, 
     for (int c = threadIdx.x; c < C; c += kEThreads) {
         float t = 0.f;
         for (int j = 0; j < rstep; ++j) t += s_part[j * C + c];
-        atomicAdd(out + c, t);
+        if (part) part[(long long)blockIdx.x * C + c] = t;
+        else atomicAdd(out + c, t);
     }
 }
 
@@ -593,14 +596,16 @@ layernorm_fwd(const T *__restrict__ x, const T *__restrict__ res, const TP *__re
 // of the y + pos output) is added to dy.  d_sum is the gradient of the LayerNorm input: it is written to
 // dres (the residual's gradient) and, times the keep-mask, to dx.  Without dropout and with dres ==
 // nullptr only dx is written.  dgamma/dbeta accumulate into fp32 buffers, one atomicAdd per channel per CTA.
-template <typename T, typename TP, int C>
+// kDet (deterministic mode): the warps are combined in index order and the CTA's [dgamma | dbeta] row is stored into
+// part[blockIdx.x] instead; partials_add_kernel then sums the rows in CTA order into dgamma / dbeta.
+template <typename T, typename TP, int C, bool kDet = false>
 __global__ void __launch_bounds__(kEThreads)
 layernorm_bwd(const T *__restrict__ x, const T *__restrict__ res, const TP *__restrict__ gamma,
               const float *__restrict__ mean_in, const float *__restrict__ rstd_in,
               const T *__restrict__ dy, const T *__restrict__ dy2, T *__restrict__ dx,
               T *__restrict__ dres, float *__restrict__ dgamma, float *__restrict__ dbeta, long long rows,
               int rows_per_cta, float drop_p, unsigned long long seed,
-              const unsigned long long *__restrict__ seed_base, long long ld2) {
+              const unsigned long long *__restrict__ seed_base, long long ld2, float *__restrict__ part = nullptr) {
     constexpr int PER = C / 32;
     constexpr int VEC = (sizeof(T) == 2) ? 8 : 4;
     if (seed_base) seed += *seed_base;
@@ -682,17 +687,47 @@ layernorm_bwd(const T *__restrict__ x, const T *__restrict__ res, const TP *__re
         }
         xr = xn; rr = rn; gr = gn; g2r = g2n;
     }
+    if constexpr (kDet) {
+        __shared__ float s_w[kStep][C];
+        for (int pass = 0; pass < 2; ++pass) {                 // dgamma, then dbeta
 #pragma unroll
-    for (int i = 0; i < PER; ++i) {
-        const int c = (i / VEC) * 32 * VEC + lane * VEC + (i % VEC);
-        atomicAdd(&s_dg[c], adg[i]);
-        atomicAdd(&s_db[c], adb[i]);
+            for (int i = 0; i < PER; ++i)
+                s_w[warp][(i / VEC) * 32 * VEC + lane * VEC + (i % VEC)] = pass ? adb[i] : adg[i];
+            __syncthreads();
+            for (int i = threadIdx.x; i < C; i += kEThreads) {
+                float t = 0.f;
+#pragma unroll
+                for (int w = 0; w < kStep; ++w) t += s_w[w][i];
+                part[((long long)blockIdx.x * 2 + pass) * C + i] = t;
+            }
+            __syncthreads();
+        }
+    } else {
+#pragma unroll
+        for (int i = 0; i < PER; ++i) {
+            const int c = (i / VEC) * 32 * VEC + lane * VEC + (i % VEC);
+            atomicAdd(&s_dg[c], adg[i]);
+            atomicAdd(&s_db[c], adb[i]);
+        }
+        __syncthreads();
+        for (int i = threadIdx.x; i < C; i += kEThreads) {
+            atomicAdd(dgamma + i, s_dg[i]);
+            atomicAdd(dbeta + i, s_db[i]);
+        }
     }
-    __syncthreads();
-    for (int i = threadIdx.x; i < C; i += kEThreads) {
-        atomicAdd(dgamma + i, s_dg[i]);
-        atomicAdd(dbeta + i, s_db[i]);
-    }
+}
+
+// Second pass of the deterministic reductions: out[c] += sum over p = 0 .. nparts-1 (in that order) of
+// part[p * width + c]; columns [0, C) go to out0, [C, width) to out1.
+__global__ void __launch_bounds__(kEThreads)
+partials_add_kernel(const float *__restrict__ part, int nparts, int width, int C, float *__restrict__ out0,
+                    float *__restrict__ out1) {
+    const int c = blockIdx.x * kEThreads + threadIdx.x;
+    if (c >= width) return;
+    float t = 0.f;
+    for (int p = 0; p < nparts; ++p) t += part[(long long)p * width + c];
+    if (c < C) out0[c] += t;
+    else out1[c - C] += t;
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -1102,33 +1137,42 @@ extern "C" int bevf_layernorm_forward(const void *x, const void *residual, const
     return fail("%s: unsupported dtype code", who);
 }
 
+// rows per CTA and grid of the LayerNorm backward, shared by the launch and the workspace query
+static unsigned ln_bwd_plan(long long rows, int &rows_per_cta) {
+    // ~4 CTAs per SM worth of row chunks keeps the per-channel atomics few
+    rows_per_cta = (int)((rows + device_sms() * 4 - 1) / (device_sms() * 4));
+    rows_per_cta = ((rows_per_cta + 7) / 8) * 8;
+    if (rows_per_cta < 8) rows_per_cta = 8;
+    return blocks_for(rows, rows_per_cta);
+}
+
 template <typename T, typename TP>
 static int ln_bwd_t(const char *who, const void *x, const void *res, const void *gamma, const float *mean,
                     const float *rstd, const void *dy, const void *dy2, void *dx, void *dres, float *dgamma,
                     float *dbeta, long long rows, int C, float drop_p, unsigned long long seed,
-                    const unsigned long long *sb, long long ld2, cudaStream_t st) {
-    // ~4 CTAs per SM worth of row chunks keeps the per-channel atomics few
-    int rows_per_cta = (int)((rows + device_sms() * 4 - 1) / (device_sms() * 4));
-    rows_per_cta = ((rows_per_cta + 7) / 8) * 8;
-    if (rows_per_cta < 8) rows_per_cta = 8;
-    const unsigned grid = blocks_for(rows, rows_per_cta);
-    if (C == 256)
-        layernorm_bwd<T, TP, 256><<<grid, kEThreads, 0, st>>>((const T *)x, (const T *)res, (const TP *)gamma, mean, rstd, (const T *)dy, (const T *)dy2, (T *)dx, (T *)dres, dgamma, dbeta, rows, rows_per_cta, drop_p, seed, sb, ld2);
-    else if (C == 512)
-        layernorm_bwd<T, TP, 512><<<grid, kEThreads, 0, st>>>((const T *)x, (const T *)res, (const TP *)gamma, mean, rstd, (const T *)dy, (const T *)dy2, (T *)dx, (T *)dres, dgamma, dbeta, rows, rows_per_cta, drop_p, seed, sb, ld2);
-    else
-        return fail("%s: embed_dims must be 256 or 512", who);
-    return check_launch(who);
+                    const unsigned long long *sb, long long ld2, cudaStream_t st, float *part = nullptr) {
+    int rows_per_cta;
+    const unsigned grid = ln_bwd_plan(rows, rows_per_cta);
+    if (C != 256 && C != 512) return fail("%s: embed_dims must be 256 or 512", who);
+    auto kernel = C == 256 ? (part ? layernorm_bwd<T, TP, 256, true> : layernorm_bwd<T, TP, 256, false>)
+                           : (part ? layernorm_bwd<T, TP, 512, true> : layernorm_bwd<T, TP, 512, false>);
+    kernel<<<grid, kEThreads, 0, st>>>((const T *)x, (const T *)res, (const TP *)gamma, mean, rstd, (const T *)dy,
+                                       (const T *)dy2, (T *)dx, (T *)dres, dgamma, dbeta, rows, rows_per_cta, drop_p, seed,
+                                       sb, ld2, part);
+    if (int e = check_launch(who)) return e;
+    if (part) {
+        partials_add_kernel<<<(unsigned)((2 * C + kEThreads - 1) / kEThreads), kEThreads, 0, st>>>(part, (int)grid, 2 * C,
+                                                                                                   C, dgamma, dbeta);
+        return check_launch(who);
+    }
+    return 0;
 }
 
-extern "C" int bevf_layernorm_backward(const void *x, const void *residual, const void *gamma,
-                                       int param_dtype, const float *mean, const float *rstd,
-                                       const void *dy, const void *dy_plus_pos, int64_t dy_plus_pos_ld, void *dx,
-                                       void *dres,
-                                       float *dgamma, float *dbeta, int64_t rows, int C, float drop_p,
-                                       uint64_t seed, const uint64_t *seed_base, int dtype,
-                                       void *stream) {
-    const char *who = "bevf_layernorm_backward";
+static int layernorm_backward_impl(const char *who, const void *x, const void *residual, const void *gamma,
+                                   int param_dtype, const float *mean, const float *rstd, const void *dy,
+                                   const void *dy_plus_pos, int64_t dy_plus_pos_ld, void *dx, void *dres, float *dgamma,
+                                   float *dbeta, int64_t rows, int C, float drop_p, uint64_t seed,
+                                   const uint64_t *seed_base, int dtype, void *stream, float *part = nullptr) {
     const unsigned long long *sb = reinterpret_cast<const unsigned long long *>(seed_base);
     BEVF_REQUIRE(rows >= 0 && C > 0, who, "bad dimension");
     if (rows == 0) return 0;
@@ -1141,13 +1185,49 @@ extern "C" int bevf_layernorm_backward(const void *x, const void *residual, cons
     BEVF_REQUIRE(pb || param_dtype == BEVF_DTYPE_F32, who, "unsupported parameter dtype code");
     if (dtype == BEVF_DTYPE_F32) {
         if (pb) return fail("%s: bf16 parameters with fp32 activations are not supported", who);
-        return ln_bwd_t<float, float>(who, x, residual, gamma, mean, rstd, dy, dy_plus_pos, dx, dres, dgamma, dbeta, rows, C, drop_p, seed, sb, ld2, st);
+        return ln_bwd_t<float, float>(who, x, residual, gamma, mean, rstd, dy, dy_plus_pos, dx, dres, dgamma, dbeta, rows, C, drop_p, seed, sb, ld2, st, part);
     }
     if (dtype == BEVF_DTYPE_BF16) {
-        if (pb) return ln_bwd_t<bf16, bf16>(who, x, residual, gamma, mean, rstd, dy, dy_plus_pos, dx, dres, dgamma, dbeta, rows, C, drop_p, seed, sb, ld2, st);
-        return ln_bwd_t<bf16, float>(who, x, residual, gamma, mean, rstd, dy, dy_plus_pos, dx, dres, dgamma, dbeta, rows, C, drop_p, seed, sb, ld2, st);
+        if (pb) return ln_bwd_t<bf16, bf16>(who, x, residual, gamma, mean, rstd, dy, dy_plus_pos, dx, dres, dgamma, dbeta, rows, C, drop_p, seed, sb, ld2, st, part);
+        return ln_bwd_t<bf16, float>(who, x, residual, gamma, mean, rstd, dy, dy_plus_pos, dx, dres, dgamma, dbeta, rows, C, drop_p, seed, sb, ld2, st, part);
     }
     return fail("%s: unsupported dtype code", who);
+}
+
+extern "C" int bevf_layernorm_backward(const void *x, const void *residual, const void *gamma,
+                                       int param_dtype, const float *mean, const float *rstd,
+                                       const void *dy, const void *dy_plus_pos, int64_t dy_plus_pos_ld, void *dx,
+                                       void *dres,
+                                       float *dgamma, float *dbeta, int64_t rows, int C, float drop_p,
+                                       uint64_t seed, const uint64_t *seed_base, int dtype,
+                                       void *stream) {
+    return layernorm_backward_impl("bevf_layernorm_backward", x, residual, gamma, param_dtype, mean, rstd, dy,
+                                   dy_plus_pos, dy_plus_pos_ld, dx, dres, dgamma, dbeta, rows, C, drop_p, seed,
+                                   seed_base, dtype, stream);
+}
+
+extern "C" int64_t bevf_layernorm_backward_workspace_bytes(int64_t rows, int C) {
+    if (rows <= 0 || C <= 0) return 0;
+    int rows_per_cta;
+    return (int64_t)ln_bwd_plan(rows, rows_per_cta) * 2 * C * sizeof(float);
+}
+
+extern "C" int bevf_layernorm_backward_det(const void *x, const void *residual, const void *gamma,
+                                           int param_dtype, const float *mean, const float *rstd,
+                                           const void *dy, const void *dy_plus_pos, int64_t dy_plus_pos_ld, void *dx,
+                                           void *dres, float *dgamma, float *dbeta, void *workspace,
+                                           int64_t workspace_bytes, int64_t rows, int C, float drop_p, uint64_t seed,
+                                           const uint64_t *seed_base, int dtype, void *stream) {
+    const char *who = "bevf_layernorm_backward_det";
+    if (rows <= 0) return layernorm_backward_impl(who, x, residual, gamma, param_dtype, mean, rstd, dy, dy_plus_pos,
+                                                  dy_plus_pos_ld, dx, dres, dgamma, dbeta, rows, C, drop_p, seed,
+                                                  seed_base, dtype, stream);
+    BEVF_REQUIRE(workspace && aligned16(workspace), who, "workspace must be a 16-byte aligned device buffer");
+    const int64_t need = bevf_layernorm_backward_workspace_bytes(rows, C);
+    if (workspace_bytes < need) return fail("%s: workspace too small (need %lld bytes)", who, need);
+    return layernorm_backward_impl(who, x, residual, gamma, param_dtype, mean, rstd, dy, dy_plus_pos, dy_plus_pos_ld,
+                                   dx, dres, dgamma, dbeta, rows, C, drop_p, seed, seed_base, dtype, stream,
+                                   reinterpret_cast<float *>(workspace));
 }
 
 extern "C" int bevf_sca_combine_forward(const void *out, const int32_t *pair_of,
@@ -1270,25 +1350,55 @@ extern "C" int bevf_sum_tensors(const void *const *srcs, int n, void *out, int64
     return check_launch(who);
 }
 
-extern "C" int bevf_colsum(const void *x, float *out, int64_t rows, int C, int dtype, void *stream) {
-    const char *who = "bevf_colsum";
+static unsigned colsum_plan(long long rows, long long &rows_per_cta) {
+    rows_per_cta = (rows + device_sms() * 4 - 1) / (device_sms() * 4);
+    if (rows_per_cta < 64) rows_per_cta = 64;
+    return blocks_for(rows, (int)rows_per_cta);
+}
+
+static int colsum_impl(const char *who, const void *x, float *out, int64_t rows, int C, int dtype, void *stream,
+                       float *part = nullptr) {
     BEVF_REQUIRE(rows >= 0 && C > 0, who, "bad dimension");
     if (rows == 0) return 0;
     BEVF_REQUIRE(x && out, who, "null pointer argument");
     const int vec = dtype == BEVF_DTYPE_BF16 ? 8 : 4;
     BEVF_REQUIRE(dtype == BEVF_DTYPE_BF16 || dtype == BEVF_DTYPE_F32, who, "unsupported dtype code");
     BEVF_REQUIRE(C % vec == 0 && C / vec <= kEThreads, who, "C must be a multiple of the vector width and <= 2048");
-    long long rows_per_cta = (rows + device_sms() * 4 - 1) / (device_sms() * 4);
-    if (rows_per_cta < 64) rows_per_cta = 64;
-    const unsigned grid = blocks_for(rows, (int)rows_per_cta);
+    long long rows_per_cta;
+    const unsigned grid = colsum_plan(rows, rows_per_cta);
     cudaStream_t st = (cudaStream_t)stream;
     const size_t sm = (size_t)(kEThreads / (C / vec)) * C * sizeof(float);
     BEVF_REQUIRE(sm <= 48 * 1024, who, "C too large for the row-lane staging");
     if (dtype == BEVF_DTYPE_BF16)
-        colsum_kernel<bf16><<<grid, kEThreads, sm, st>>>((const bf16 *)x, out, rows, C, (int)rows_per_cta);
+        colsum_kernel<bf16><<<grid, kEThreads, sm, st>>>((const bf16 *)x, out, rows, C, (int)rows_per_cta, part);
     else
-        colsum_kernel<float><<<grid, kEThreads, sm, st>>>((const float *)x, out, rows, C, (int)rows_per_cta);
-    return check_launch(who);
+        colsum_kernel<float><<<grid, kEThreads, sm, st>>>((const float *)x, out, rows, C, (int)rows_per_cta, part);
+    if (int e = check_launch(who)) return e;
+    if (part) {
+        partials_add_kernel<<<blocks_for(C, kEThreads), kEThreads, 0, st>>>(part, (int)grid, C, C, out, nullptr);
+        return check_launch(who);
+    }
+    return 0;
+}
+
+extern "C" int bevf_colsum(const void *x, float *out, int64_t rows, int C, int dtype, void *stream) {
+    return colsum_impl("bevf_colsum", x, out, rows, C, dtype, stream);
+}
+
+extern "C" int64_t bevf_colsum_workspace_bytes(int64_t rows, int C) {
+    if (rows <= 0 || C <= 0) return 0;
+    long long rows_per_cta;
+    return (int64_t)colsum_plan(rows, rows_per_cta) * C * sizeof(float);
+}
+
+extern "C" int bevf_colsum_det(const void *x, float *out, void *workspace, int64_t workspace_bytes, int64_t rows, int C,
+                               int dtype, void *stream) {
+    const char *who = "bevf_colsum_det";
+    if (rows <= 0) return colsum_impl(who, x, out, rows, C, dtype, stream);
+    BEVF_REQUIRE(workspace && aligned16(workspace), who, "workspace must be a 16-byte aligned device buffer");
+    const int64_t need = bevf_colsum_workspace_bytes(rows, C);
+    if (workspace_bytes < need) return fail("%s: workspace too small (need %lld bytes)", who, need);
+    return colsum_impl(who, x, out, rows, C, dtype, stream, reinterpret_cast<float *>(workspace));
 }
 
 extern "C" int bevf_relu_dropout_backward(const void *dy, const void *h, void *out, int64_t n, float scale,

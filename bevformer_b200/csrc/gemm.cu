@@ -614,11 +614,13 @@ gemm_ws_wgmma(const __grid_constant__ CUtensorMap map_a, const __grid_constant__
 }
 
 // second pass of the two-pass weight gradient: dW[n, k] = sum over splits of the partial slabs, written
-// in the parameter's own dtype (no zero-fill, no cast kernel); db likewise.
-template <typename TO>
+// in the parameter's own dtype (no zero-fill, no cast kernel); db likewise.  kAcc: dw / db (fp32) are added into.
+// The slabs are summed in split order, so the result does not depend on how the splits were scheduled.
+template <typename TO, bool kAcc = false>
 __global__ void __launch_bounds__(256)
 wgrad_reduce_kernel(const float *__restrict__ ws, const float *__restrict__ ws_b, TO *__restrict__ dw,
                     TO *__restrict__ db, int N, int K, int n_pad, int splits) {
+    static_assert(!kAcc || sizeof(TO) == 4, "accumulation into fp32 only");
     const int kv = K / 4;
     const long long t = (long long)blockIdx.x * blockDim.x + threadIdx.x;
     const long long total = (long long)N * kv;
@@ -634,6 +636,10 @@ wgrad_reduce_kernel(const float *__restrict__ ws, const float *__restrict__ ws_b
         }
         if constexpr (sizeof(TO) == 2) {
             *reinterpret_cast<uint2 *>(dw + (size_t)n * K + c) = make_uint2(pack_bf16x2(a.x, a.y), pack_bf16x2(a.z, a.w));
+        } else if constexpr (kAcc) {
+            float4 *d = reinterpret_cast<float4 *>(dw + (size_t)n * K + c);
+            const float4 o = *d;
+            *d = make_float4(o.x + a.x, o.y + a.y, o.z + a.z, o.w + a.w);
         } else {
             *reinterpret_cast<float4 *>(dw + (size_t)n * K + c) = a;
         }
@@ -641,7 +647,9 @@ wgrad_reduce_kernel(const float *__restrict__ ws, const float *__restrict__ ws_b
         const int n = (int)(t - total);
         float a = 0.f;
         for (int s2 = 0; s2 < splits; ++s2) a += ws_b[(size_t)s2 * n_pad + n];
-        if constexpr (sizeof(TO) == 2) db[n] = __float2bfloat16_rn(a); else db[n] = a;
+        if constexpr (sizeof(TO) == 2) db[n] = __float2bfloat16_rn(a);
+        else if constexpr (kAcc) db[n] += a;
+        else db[n] = a;
     }
 }
 
@@ -914,10 +922,10 @@ extern "C" int64_t bevf_linear_wgrad_workspace_bytes(int64_t M, int N, int K) {
     return (int64_t)splits * n_pad * ((int64_t)K + 1) * 4 + 256;
 }
 
-extern "C" int bevf_linear_wgrad_out(const void *dy, const void *x, void *dw, void *db, int grad_dtype,
-                                     void *workspace, int64_t workspace_bytes, int64_t M, int N, int K,
-                                     void *stream) {
-    const char *who = "bevf_linear_wgrad_out";
+// grad_dtype, or accumulate != 0: dw / db fp32 and added into
+static int wgrad_two_pass(const char *who, const void *dy, const void *x, void *dw, void *db, int grad_dtype,
+                          int accumulate, void *workspace, int64_t workspace_bytes, int64_t M, int N, int K,
+                          void *stream) {
     if (M <= 0 || N <= 0 || K <= 0) return fail("%s: bad dimension", who);
     if (!dy || !x || !dw || !workspace) return fail("%s: null pointer argument", who);
     if (K % 64 != 0 || N % 8 != 0) return fail("%s: K must be a multiple of 64 and N of 8", who);
@@ -941,9 +949,24 @@ extern "C" int bevf_linear_wgrad_out(const void *dy, const void *x, void *dw, vo
     // pass 2: sum the slabs in the parameter's dtype
     const long long total = (long long)N * (K / 4) + (db ? N : 0);
     const unsigned rgrid = (unsigned)((total + 255) / 256);
-    if (grad_dtype == BEVF_DTYPE_BF16)
+    if (accumulate)
+        wgrad_reduce_kernel<float, true><<<rgrid, 256, 0, cs>>>(ws, ws_b, (float *)dw, (float *)db, N, K, n_pad, splits);
+    else if (grad_dtype == BEVF_DTYPE_BF16)
         wgrad_reduce_kernel<bf16><<<rgrid, 256, 0, cs>>>(ws, ws_b, (bf16 *)dw, (bf16 *)db, N, K, n_pad, splits);
     else
         wgrad_reduce_kernel<float><<<rgrid, 256, 0, cs>>>(ws, ws_b, (float *)dw, (float *)db, N, K, n_pad, splits);
     return check_launch(who);
+}
+
+extern "C" int bevf_linear_wgrad_out(const void *dy, const void *x, void *dw, void *db, int grad_dtype,
+                                     void *workspace, int64_t workspace_bytes, int64_t M, int N, int K,
+                                     void *stream) {
+    return wgrad_two_pass("bevf_linear_wgrad_out", dy, x, dw, db, grad_dtype, 0, workspace, workspace_bytes, M, N, K,
+                          stream);
+}
+
+extern "C" int bevf_linear_wgrad_into(const void *dy, const void *x, float *dw, float *db, void *workspace,
+                                      int64_t workspace_bytes, int64_t M, int N, int K, void *stream) {
+    return wgrad_two_pass("bevf_linear_wgrad_into", dy, x, dw, db, BEVF_DTYPE_F32, 1, workspace, workspace_bytes, M, N,
+                          K, stream);
 }

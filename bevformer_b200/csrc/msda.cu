@@ -139,7 +139,11 @@ msda_bwd_d32(const T *__restrict__ value, const int64_t *__restrict__ level_hw,
              float *__restrict__ grad_attn, const int *__restrict__ row_map, int S, int M, int Q,
              int L, int P, int magic, int iters, long long rows, unsigned red_skip,
              const __grid_constant__ HostLevels host_levels, const unsigned *__restrict__ gv_amax = nullptr,
-             __half *__restrict__ gv16 = nullptr, unsigned gv16_mask = 0u, int side_start = 0, int S_side = 0) {
+             __half *__restrict__ gv16 = nullptr, unsigned gv16_mask = 0u, int side_start = 0, int S_side = 0,
+             const unsigned *__restrict__ fx_bounds = nullptr, int fx_bits = 0) {
+    // TV = long long: grad_value in 64-bit fixed point (deterministic mode): each lane adds VEC channels of every
+    // corner contribution with scalar integer reductions, scaled by 2^(fx_bits - fx_exponent(fx_bounds)) (common.cuh);
+    // non-finite bounds: nothing is scattered (the conversion then writes NaN)
     // Mixed accumulation (gv16 != nullptr, TV = float): the levels of gv16_mask -- the fine ones, pixels
     // [0, side_start) of every map, where a pixel collects few contributions -- are accumulated in scaled fp16 into
     // gv16 (B, side_start, M, 32); the other levels are the pixels [side_start, S) and accumulate in fp32 into
@@ -170,6 +174,13 @@ msda_bwd_d32(const T *__restrict__ value, const int64_t *__restrict__ level_hw,
     red_skip = s_skip;
     if (gv16 != nullptr) gv16_mask = s_mask16;
     const float gv_sc = gv_amax ? gv16_scale(__ldg(gv_amax)) : 1.f;       // scale of the fp16 accumulators
+    constexpr bool kGvFx = sizeof(TV) == 8;
+    double fx_sc = 0.0;
+    if constexpr (kGvFx) {
+        const unsigned ba = __ldg(fx_bounds), bg = __ldg(fx_bounds + 1);
+        if (fx_bounds_finite(ba, bg)) fx_sc = fx_pow2(fx_bits - fx_exponent(ba, bg));
+        else red_skip = ~0u;
+    }
 
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
     const int sub = lane % LANES, grp = lane / LANES;
@@ -192,6 +203,11 @@ msda_bwd_d32(const T *__restrict__ value, const int64_t *__restrict__ level_hw,
     uint4 gh = make_uint4(0, 0, 0, 0);            // the same slice as packed bf16, for the fhfma dots
     if constexpr (kHalfDot)
         gh = __ldg(reinterpret_cast<const uint4 *>(grad_out + row * 32 + sub * VEC));
+    float gx[kGvFx ? VEC : 1];                    // fixed-point scatter: channels k * LANES + sub of the row
+    if constexpr (kGvFx) {
+#pragma unroll
+        for (int k = 0; k < VEC; ++k) gx[k] = Row<TG>::load1(grad_out + row * 32 + k * LANES + sub);
+    }
     // Scatter layout.  A 16 B reduction covers 4 fp32 channels and the reduction path is fastest
     // when one warp instruction fills whole 128 B lines rather than half lines.  VEC == 4: the 8 lanes of a
     // row already write its 128 B.
@@ -202,7 +218,7 @@ msda_bwd_d32(const T *__restrict__ value, const int64_t *__restrict__ level_hw,
     // partner's per-sample scalars with one extra shuffle each.
     constexpr bool kGvHalf = sizeof(TV) == 2;
     static_assert(!kGvHalf || VEC == 8, "fp16 grad_value needs bf16 value rows (8 channels per lane)");
-    constexpr bool kPaired = (VEC == 8) && kScatter && !kGvHalf;
+    constexpr bool kPaired = (VEC == 8) && kScatter && !kGvHalf && !kGvFx;
     const bool hi = kPaired && (grp & 4);
     const long long vrow = voff - sub * VEC;                       // element offset of the row in its map
     long long vrow_a = vrow, vrow_b = vrow;
@@ -280,6 +296,18 @@ msda_bwd_d32(const T *__restrict__ value, const int64_t *__restrict__ level_hw,
             // scatter w * a * g with 16 B reductions; zero-weight corners are skipped
             if constexpr (!kScatter) {
             } else if ((red_skip >> l) & 1u) {
+            } else if constexpr (kGvFx) {
+                // lane `sub` adds channels k * LANES + sub (gx): in each of the VEC instructions the LANES lanes of a row
+                // write adjacent 8-byte words, i.e. whole 32-byte sectors
+                long long *gp = reinterpret_cast<long long *>(grad_value) + (o00 - sub * VEC) + sub;
+                auto redfx = [&](long long *p, float q) {
+#pragma unroll
+                    for (int k = 0; k < VEC; ++k) red_add_fx(p + k * LANES, q, gx[k], fx_sc);
+                };
+                if (q00 != 0.f) redfx(gp, q00);
+                if (q01 != 0.f) redfx(gp + ox, q01);
+                if (q10 != 0.f) redfx(gp + oy, q10);
+                if (q11 != 0.f) redfx(gp + oy + ox, q11);
             } else if constexpr (kGvHalf) {
                 // scaled fp16 accumulation: this lane's 8 channels of the row as one 16-byte f16x2 vector reduction
                 TV *gp = grad_value + o00;
@@ -415,16 +443,26 @@ msda_fwd_generic(const T *__restrict__ value, const int64_t *__restrict__ level_
     }
 }
 
-template <typename T, typename TG>
+// TV = long long: grad_value in 64-bit fixed point, as in msda_bwd_d32
+template <typename T, typename TG, typename TV = float>
 __global__ void __launch_bounds__(kThreads)
 msda_bwd_generic(const T *__restrict__ value, const int64_t *__restrict__ level_hw,
                  const int64_t *__restrict__ level_start, const float *__restrict__ loc,
                  const float *__restrict__ attn, const TG *__restrict__ grad_out,
-                 float *__restrict__ grad_value, float *__restrict__ grad_loc,
+                 TV *__restrict__ grad_value, float *__restrict__ grad_loc,
                  float *__restrict__ grad_attn, const int *__restrict__ row_map, int S, int M,
-                 int D, int Q, int L, int P, long long rows) {
+                 int D, int Q, int L, int P, long long rows,
+                 const unsigned *__restrict__ fx_bounds = nullptr, int fx_bits = 0) {
     __shared__ int s_h[kMaxLevels], s_w[kMaxLevels], s_start[kMaxLevels];
     load_levels(level_hw, level_start, L, s_h, s_w, s_start);
+    constexpr bool kGvFx = sizeof(TV) == 8;
+    double fx_sc = 0.0;
+    bool scatter = true;
+    if constexpr (kGvFx) {
+        const unsigned ba = __ldg(fx_bounds), bg = __ldg(fx_bounds + 1);
+        scatter = fx_bounds_finite(ba, bg);
+        if (scatter) fx_sc = fx_pow2(fx_bits - fx_exponent(ba, bg));
+    }
     const int lane = threadIdx.x & 31;
     const long long row = (long long)blockIdx.x * (kThreads / 32) + (threadIdx.x >> 5);
     if (row >= rows) return;   // whole warp leaves together
@@ -450,10 +488,19 @@ msda_bwd_generic(const T *__restrict__ value, const int64_t *__restrict__ level_
                 const float v01 = c.f01 * Row<T>::load1(value + i01 + c0);
                 const float v10 = c.f10 * Row<T>::load1(value + i10 + c0);
                 const float v11 = c.f11 * Row<T>::load1(value + i11 + c0);
-                if (c.w00 != 0.f) atomicAdd(grad_value + i00 + c0, c.w00 * t);
-                if (c.w01 != 0.f) atomicAdd(grad_value + i01 + c0, c.w01 * t);
-                if (c.w10 != 0.f) atomicAdd(grad_value + i10 + c0, c.w10 * t);
-                if (c.w11 != 0.f) atomicAdd(grad_value + i11 + c0, c.w11 * t);
+                if constexpr (kGvFx) {
+                    if (scatter) {
+                        if (c.w00 != 0.f) red_add_fx(grad_value + i00 + c0, c.w00 * a, gc, fx_sc);
+                        if (c.w01 != 0.f) red_add_fx(grad_value + i01 + c0, c.w01 * a, gc, fx_sc);
+                        if (c.w10 != 0.f) red_add_fx(grad_value + i10 + c0, c.w10 * a, gc, fx_sc);
+                        if (c.w11 != 0.f) red_add_fx(grad_value + i11 + c0, c.w11 * a, gc, fx_sc);
+                    }
+                } else {
+                    if (c.w00 != 0.f) atomicAdd(grad_value + i00 + c0, c.w00 * t);
+                    if (c.w01 != 0.f) atomicAdd(grad_value + i01 + c0, c.w01 * t);
+                    if (c.w10 != 0.f) atomicAdd(grad_value + i10 + c0, c.w10 * t);
+                    if (c.w11 != 0.f) atomicAdd(grad_value + i11 + c0, c.w11 * t);
+                }
                 ga += gc * (hy * (hx * v00 + c.lx * v01) + c.ly * (hx * v10 + c.lx * v11));
                 gx += t * (hy * (v01 - v00) + c.ly * (v11 - v10));
                 gy += t * (hx * (v10 - v00) + c.lx * (v11 - v01));
@@ -594,15 +641,39 @@ struct MixedGv {               // scaled-fp16 / mixed accumulation of grad_value
     int side_start = 0, S_side = 0;
 };
 
+struct FxGv {                  // 64-bit fixed-point grad_value (deterministic mode)
+    const unsigned *bounds = nullptr;        // max|attn|, max|grad_out| bits (gvfx.cu: fx_bounds)
+    int frac_bits = 0;
+};
+
 template <typename T, typename TG>
 static int launch_bwd(const char *who, const void *value, const int64_t *hw, const int64_t *ls,
                       const float *loc, const float *attn, const void *go, float *gv, float *gl,
                       float *ga, const int *row_map, const int *order, int S, int M, int D, int Q,
                       int L, int P, long long rows, cudaStream_t st, unsigned done_levels = 0,
                       const HostLevels *host_levels = nullptr, bool gv_f16 = false,
-                      const MixedGv *mixed = nullptr) {
+                      const MixedGv *mixed = nullptr, const FxGv *fx = nullptr) {
     HostLevels hl;
     if (host_levels) hl = *host_levels; else memset(&hl, 0, sizeof(hl));
+    if (fx) {
+        // fixed-point grad_value: always the one-kernel backward (the split / hybrid / dense modes sum in fp32)
+        long long *gfx = reinterpret_cast<long long *>(gv);
+        if (D == 32) {
+            constexpr int G = Vec<T>::N;
+            const int iters = pick_iters(rows, G);
+            const long long per_block = (long long)(kThreads / 32) * G * iters;
+            const unsigned grid = (unsigned)((rows + per_block - 1) / per_block);
+            msda_bwd_d32<T, TG, true, long long><<<grid, kThreads, 0, st>>>(
+                (const T *)value, hw, ls, loc, attn, (const TG *)go, gfx, gl, ga, row_map, S, M, Q, L, P,
+                (65536 + P - 1) / P, iters, rows, 0u, hl, nullptr, nullptr, 0u, 0, 0, fx->bounds, fx->frac_bits);
+        } else {
+            const unsigned grid = (unsigned)((rows + kThreads / 32 - 1) / (kThreads / 32));
+            msda_bwd_generic<T, TG, long long><<<grid, kThreads, 0, st>>>(
+                (const T *)value, hw, ls, loc, attn, (const TG *)go, gfx, gl, ga, row_map, S, M, D, Q, L, P, rows,
+                fx->bounds, fx->frac_bits);
+        }
+        return check_launch(who);
+    }
     if (gv_f16) {
         // grad_value stored and accumulated in scaled fp16: bf16 value rows, head_dim 32, the one-kernel backward only
         if constexpr (sizeof(T) == 2) {
@@ -710,7 +781,7 @@ static int msda_backward_impl(const char *who, const void *value, int value_dtyp
                               const int *row_map, const int *order, int B, int S, int M, int D, int Q,
                               int L, int P, void *stream, unsigned done_levels = 0,
                               const HostLevels *host_levels = nullptr, bool gv_f16 = false,
-                              const MixedGv *mixed = nullptr) {
+                              const MixedGv *mixed = nullptr, const FxGv *fx = nullptr) {
     if (int e = check_dims(who, B, S, M, D, Q, L, P)) return e;
     const long long rows = (row_map ? 1ll : (long long)B) * Q * M;
     if (rows == 0) return 0;
@@ -724,9 +795,9 @@ static int msda_backward_impl(const char *who, const void *value, int value_dtyp
     const bool vb = value_dtype == BEVF_DTYPE_BF16, gb = grad_out_dtype == BEVF_DTYPE_BF16;
     if ((value_dtype != BEVF_DTYPE_F32 && !vb) || (grad_out_dtype != BEVF_DTYPE_F32 && !gb))
         return fail("%s: unsupported dtype code", who);
-    if (!vb && !gb) return launch_bwd<float, float>(who, value, level_hw, level_start, loc, attn, grad_out, grad_value, grad_loc, grad_attn, row_map, order, S, M, D, Q, L, P, rows, st, done_levels, host_levels, gv_f16, mixed);
-    if (vb && gb) return launch_bwd<bf16, bf16>(who, value, level_hw, level_start, loc, attn, grad_out, grad_value, grad_loc, grad_attn, row_map, order, S, M, D, Q, L, P, rows, st, done_levels, host_levels, gv_f16, mixed);
-    if (vb && !gb) return launch_bwd<bf16, float>(who, value, level_hw, level_start, loc, attn, grad_out, grad_value, grad_loc, grad_attn, row_map, order, S, M, D, Q, L, P, rows, st, done_levels, host_levels, gv_f16, mixed);
+    if (!vb && !gb) return launch_bwd<float, float>(who, value, level_hw, level_start, loc, attn, grad_out, grad_value, grad_loc, grad_attn, row_map, order, S, M, D, Q, L, P, rows, st, done_levels, host_levels, gv_f16, mixed, fx);
+    if (vb && gb) return launch_bwd<bf16, bf16>(who, value, level_hw, level_start, loc, attn, grad_out, grad_value, grad_loc, grad_attn, row_map, order, S, M, D, Q, L, P, rows, st, done_levels, host_levels, gv_f16, mixed, fx);
+    if (vb && !gb) return launch_bwd<bf16, float>(who, value, level_hw, level_start, loc, attn, grad_out, grad_value, grad_loc, grad_attn, row_map, order, S, M, D, Q, L, P, rows, st, done_levels, host_levels, gv_f16, mixed, fx);
     return fail("%s: fp32 value with bf16 grad_out is not supported", who);
 }
 
@@ -905,6 +976,58 @@ extern "C" int bevf_msda_rows_backward_mixed(const void *value, int value_dtype,
     return msda_backward_impl(who, value, value_dtype, level_hw, level_start, loc, attn, grad_out, grad_out_dtype,
                               grad_value_side, grad_loc, grad_attn, row_map, group_order, B, S, M, D, R, L, P, stream, 0u,
                               &hl, false, &mx);
+}
+
+namespace bevf {
+int fx_bounds_launch(const char *who, const float *attn, const void *grad_out, int grad_out_dtype,
+                     const int32_t *row_map, long long qrows, int M, int D, int L, int P, uint32_t *bounds,
+                     cudaStream_t st);                                                    // gvfx.cu
+
+// Deterministic backward: the bounds of this launch, then the fixed-point scatter.  rows_per_map (Q, or R for a row
+// list) caps the contributions one element can receive; frac_bits above what that allows could overflow.
+static int msda_backward_fx_impl(const char *who, const void *value, int value_dtype, const int64_t *level_hw,
+                                 const int64_t *level_start, const float *loc, const float *attn, const void *grad_out,
+                                 int grad_out_dtype, int64_t *grad_value_fx, uint32_t *bounds, int frac_bits,
+                                 float *grad_loc, float *grad_attn, const int32_t *row_map, int B, int S, int M, int D,
+                                 int Q, int L, int P, void *stream) {
+    if (int e = check_dims(who, B, S, M, D, Q, L, P)) return e;
+    const long long qrows = (row_map ? 1ll : (long long)B) * Q;
+    if (qrows == 0) return 0;
+    if (!bounds || !grad_value_fx || !attn || !grad_out) return fail("%s: null pointer argument", who);
+    const int kmax = bevf_msda_fx_frac_bits(Q, L, P);
+    if (frac_bits < 0 || frac_bits > kmax)
+        return fail("%s: frac_bits must be in [0, %lld] for this launch (bevf_msda_fx_frac_bits)", who, kmax);
+    cudaStream_t st = (cudaStream_t)stream;
+    if (int e = fx_bounds_launch(who, attn, grad_out, grad_out_dtype, row_map, qrows, M, D, L, P, bounds, st)) return e;
+    FxGv fx;
+    fx.bounds = bounds;
+    fx.frac_bits = frac_bits;
+    return msda_backward_impl(who, value, value_dtype, level_hw, level_start, loc, attn, grad_out, grad_out_dtype,
+                              reinterpret_cast<float *>(grad_value_fx), grad_loc, grad_attn, row_map, nullptr, B, S, M,
+                              D, Q, L, P, stream, 0u, nullptr, false, nullptr, &fx);
+}
+}  // namespace bevf
+
+extern "C" int bevf_msda_backward_fx(const void *value, int value_dtype, const int64_t *level_hw,
+                                     const int64_t *level_start, const float *loc, const float *attn,
+                                     const void *grad_out, int grad_out_dtype, int64_t *grad_value_fx,
+                                     uint32_t *bounds, int frac_bits, float *grad_loc, float *grad_attn, int B, int S,
+                                     int M, int D, int Q, int L, int P, void *stream) {
+    return msda_backward_fx_impl("bevf_msda_backward_fx", value, value_dtype, level_hw, level_start, loc, attn, grad_out,
+                                 grad_out_dtype, grad_value_fx, bounds, frac_bits, grad_loc, grad_attn, nullptr, B, S, M,
+                                 D, Q, L, P, stream);
+}
+
+extern "C" int bevf_msda_rows_backward_fx(const void *value, int value_dtype, const int64_t *level_hw,
+                                          const int64_t *level_start, const float *loc, const float *attn,
+                                          const void *grad_out, int grad_out_dtype, int64_t *grad_value_fx,
+                                          uint32_t *bounds, int frac_bits, float *grad_loc, float *grad_attn,
+                                          const int32_t *row_map, int B, int S, int M, int D, int R, int L, int P,
+                                          void *stream) {
+    if (!row_map && R > 0) return fail("%s: row_map is null", "bevf_msda_rows_backward_fx");
+    return msda_backward_fx_impl("bevf_msda_rows_backward_fx", value, value_dtype, level_hw, level_start, loc, attn,
+                                 grad_out, grad_out_dtype, grad_value_fx, bounds, frac_bits, grad_loc, grad_attn, row_map,
+                                 B, S, M, D, R, L, P, stream);
 }
 
 extern "C" int bevf_msda_set_backward_mode(int mode) {

@@ -8,6 +8,7 @@ the current stream only; all arithmetic happens in ``libbevformer_b200.so``.
 from __future__ import annotations
 
 import os
+import warnings
 
 import torch
 from torch.autograd.function import Function, once_differentiable
@@ -16,6 +17,26 @@ from . import _lib
 
 F32, BF16 = 0, 1
 _DT = {torch.float32: F32, torch.bfloat16: BF16}
+
+
+def deterministic() -> bool:
+    """``torch.use_deterministic_algorithms(True)`` is in effect: every backward of this package that would sum
+    through atomics (sampler grad_value, LayerNorm dgamma / dbeta, bias column sums, weight gradients) takes its
+    fixed-order kernel instead, and results repeat bit for bit from run to run on one GPU model."""
+    return torch.are_deterministic_algorithms_enabled()
+
+
+def alert_not_deterministic(name: str) -> None:
+    """PyTorch's contract for an op without a deterministic implementation: raise under
+    ``torch.use_deterministic_algorithms(True)``, warn under ``warn_only=True``."""
+    if not torch.are_deterministic_algorithms_enabled():
+        return
+    msg = (f"{name} does not have a deterministic implementation, but you set "
+           "'torch.use_deterministic_algorithms(True)'.")
+    if torch.is_deterministic_algorithms_warn_only_enabled():
+        warnings.warn(msg)
+    else:
+        raise RuntimeError(msg)
 
 # bench.py's roofline needs the duration of individual launches inside the timed region: when a name
 # is present in KERNEL_TIMERS, the wrapper brackets that launch with CUDA events on the launching
@@ -118,6 +139,10 @@ def msda_backward(value, spatial_shapes, level_start_index, sampling_locations, 
         grad_value = torch.zeros(value.shape, device=value.device, dtype=torch.float32)
     elif grad_value.dtype != torch.float32 or tuple(grad_value.shape) != tuple(value.shape):
         raise RuntimeError("grad_value must be float32 with value's shape")
+    if deterministic():
+        gv, grad_loc, grad_attn = msda_backward_fx(value, ss, ls, loc, attn, grad_output)
+        gv.add_into(grad_value)
+        return grad_value, grad_loc, grad_attn
     grad_loc = torch.empty(loc.shape, device=value.device, dtype=torch.float32)
     grad_attn = torch.empty(attn.shape, device=value.device, dtype=torch.float32)
     lib = _lib.load()
@@ -275,6 +300,11 @@ def msda_rows_backward(value, spatial_shapes, level_start_index, loc, attn, row_
     ss, ls = _level_tensors(value, spatial_shapes, level_start_index)
     if grad_value is None:
         grad_value = torch.zeros(value.shape, device=value.device, dtype=torch.float32)
+    if deterministic():
+        # fixed point sums in any order: group_order has nothing to merge, and the dense kernel sums in fp32
+        gv, grad_loc, grad_attn = msda_backward_fx(value, ss, ls, loc, attn, grad_output, row_map)
+        gv.add_into(grad_value)
+        return grad_value, grad_loc, grad_attn
     grad_loc = torch.empty(loc.shape, device=value.device, dtype=torch.float32)
     grad_attn = torch.empty(attn.shape, device=value.device, dtype=torch.float32)
     lib = _lib.load()
@@ -356,6 +386,76 @@ class LazyGradValue:
         return gv
 
 
+class FixedPointGradValue(LazyGradValue):
+    """grad_value of the deterministic sampler backward, still as int64 fixed-point sums (bevf_msda_backward_fx):
+    ``materialize()`` converts it into a new tensor of ``dtype`` (the value's), ``add_into(t)`` adds it into an fp32
+    buffer; both on the CURRENT stream, so the conversion can run off the critical path like LazyGradValue's."""
+
+    def __init__(self, fx, bounds, frac_bits, dtype):
+        self.shape, self.fx, self.bounds, self.frac_bits, self.dtype = tuple(fx.shape), fx, bounds, frac_bits, dtype
+        self.tensors = (fx, bounds)
+        self.device = fx.device
+
+    def _convert(self, out, accumulate):
+        lib = _lib.load()
+        with torch.cuda.device(self.device):
+            st = lib.bevf_msda_fx_convert(self.fx.data_ptr(), self.bounds.data_ptr(), self.frac_bits, out.data_ptr(),
+                                          _DT[out.dtype], int(accumulate), out.numel(), _stream_ptr(out))
+        _lib.check(st, lib)
+        return out
+
+    def materialize(self) -> torch.Tensor:
+        return self._convert(torch.empty(self.shape, device=self.device, dtype=self.dtype), False)
+
+    def add_into(self, out: torch.Tensor) -> torch.Tensor:
+        if out.dtype not in _DT or tuple(out.shape) != self.shape or not out.is_contiguous():
+            raise RuntimeError("add_into: a contiguous float32 / bfloat16 tensor of grad_value's shape is required")
+        return self._convert(out, True)
+
+
+def msda_backward_fx(value, spatial_shapes, level_start_index, loc, attn, grad_output, row_map=None):
+    """Deterministic sampler backward (bevf_msda_backward_fx / bevf_msda_rows_backward_fx): grad_value summed in
+    64-bit fixed point, whatever the order of the rows.  Plain form: loc (B, Q, M, L, P, 2), grad_output (B, Q, M*D);
+    row-list form (``row_map`` (R,) int32): loc (R, M, L, P, 2), grad_output (R, M*D).  Returns (FixedPointGradValue,
+    grad_loc f32, grad_attn f32); grad_loc / grad_attn equal those of msda_backward / msda_rows_backward bit for bit."""
+    for t, n in ((value, "value"), (loc, "sampling_loc"), (attn, "attn_weight"), (grad_output, "grad_output")):
+        _need_cuda(t, n)
+    if value.dtype not in _DT or grad_output.dtype not in _DT:
+        raise RuntimeError("value / grad_output must be float32 or bfloat16")
+    loc = loc if loc.dtype == torch.float32 else loc.float()
+    attn = attn if attn.dtype == torch.float32 else attn.float()
+    NB, S, M, D = value.shape
+    if row_map is None:
+        B, S, M, D, Q, L, P = _dims(value, loc, attn)
+        if grad_output.numel() != B * Q * M * D:
+            raise RuntimeError("grad_output must be (B, Q, M*D)")
+    else:
+        _need_cuda(row_map, "row_map")
+        Q, _, L, P, _ = loc.shape
+        if (row_map.dtype != torch.int32 or row_map.numel() != Q or tuple(attn.shape) != (Q, M, L, P)
+                or grad_output.numel() != Q * M * D):
+            raise RuntimeError("value / sampling_loc / attn_weight / row_map / grad_output shapes disagree")
+    rows_per_map = Q
+    ss, ls = _level_tensors(value, spatial_shapes, level_start_index)
+    lib = _lib.load()
+    k = int(lib.bevf_msda_fx_frac_bits(rows_per_map, L, P))
+    fx = torch.zeros(value.shape, device=value.device, dtype=torch.int64)
+    bounds = torch.empty(2, device=value.device, dtype=torch.int32)
+    grad_loc = torch.empty(loc.shape, device=value.device, dtype=torch.float32)
+    grad_attn = torch.empty(attn.shape, device=value.device, dtype=torch.float32)
+    name = "msda_backward" if row_map is None else "msda_rows_backward"
+    with torch.cuda.device(value.device), _timed(name, value.device, None if row_map is None else (Q, L)):
+        args = (value.data_ptr(), _DT[value.dtype], ss.data_ptr(), ls.data_ptr(), loc.data_ptr(), attn.data_ptr(),
+                grad_output.data_ptr(), _DT[grad_output.dtype], fx.data_ptr(), bounds.data_ptr(), k,
+                grad_loc.data_ptr(), grad_attn.data_ptr())
+        if row_map is None:
+            st = lib.bevf_msda_backward_fx(*args, NB, S, M, D, Q, L, P, _stream_ptr(value))
+        else:
+            st = lib.bevf_msda_rows_backward_fx(*args, row_map.data_ptr(), NB, S, M, D, Q, L, P, _stream_ptr(value))
+    _lib.check(st, lib)
+    return FixedPointGradValue(fx, bounds, k, value.dtype), grad_loc, grad_attn
+
+
 def abs_max_bits(x: torch.Tensor) -> torch.Tensor:
     """(1,) int32 device word holding the float bits of max|x| (bevf_abs_max): the scale source of the fp16-accumulated
     sampler backward."""
@@ -377,6 +477,7 @@ def msda_rows_backward_f16acc(value, spatial_shapes, level_start_index, loc, att
     for t, n in ((value, "value"), (loc, "sampling_loc"), (attn, "attn_weight"), (row_map, "row_map"),
                  (grad_output, "grad_output")):
         _need_cuda(t, n)
+    alert_not_deterministic("msda_rows_backward_f16acc (grad_value summed with fp16 atomics)")
     if value.dtype != torch.bfloat16 or value.shape[-1] != 32:
         raise RuntimeError("fp16-accumulated backward: value must be bfloat16 with head_dim 32")
     NB, S, M, D = value.shape
@@ -409,6 +510,7 @@ def msda_rows_backward_mixed(value, spatial_shapes, level_start_index, level_hw_
     for t, n in ((value, "value"), (loc, "sampling_loc"), (attn, "attn_weight"), (row_map, "row_map"),
                  (grad_output, "grad_output")):
         _need_cuda(t, n)
+    alert_not_deterministic("msda_rows_backward_mixed (grad_value summed with fp16 / fp32 atomics)")
     if value.dtype != torch.bfloat16 or value.shape[-1] != 32:
         raise RuntimeError("mixed-accumulation backward: value must be bfloat16 with head_dim 32")
     NB, S, M, D = value.shape
@@ -491,6 +593,13 @@ class SamplerRows(Function):
     @once_differentiable
     def backward(ctx, grad_out):
         value, loc, attn, row_map, ss, ls = ctx.saved_tensors
+        if deterministic():
+            # fixed-point grad_value; gv_mode, the dense / split kernels and the pre-filled fp32 buffer all sum in
+            # floating point and are bypassed
+            gv, gl, ga = msda_backward_fx(value, ss, ls, loc, attn, grad_out.contiguous(), row_map)
+            if ctx.value_early is not None and ctx.value_early(gv):
+                return None, gl, ga, None, None, None, None, None, None      # converted off the critical path
+            return gv.materialize(), gl, ga, None, None, None, None, None, None
         gv0 = None
         if ctx.gv_zero is not None:
             gv0, done = ctx.gv_zero
@@ -746,12 +855,15 @@ class LayerNormResidual(Function):
             dgb = torch.zeros(2, C, device=x.device, dtype=torch.float32)
         lib = _lib.load()
         with torch.cuda.device(x.device):
-            st = lib.bevf_layernorm_backward(x.data_ptr(), _ptr(res), g.data_ptr(), pd, mean.data_ptr(),
-                                             rstd.data_ptr(), dy.data_ptr(), _ptr(dy2), ld2, dx.data_ptr(),
-                                             _ptr(dres), dgb[0].data_ptr(), dgb[1].data_ptr(), rows, C,
-                                             drop_p, seed,
-                                             _ptr(ctx.sbase) if drop_p > 0.0 else 0,
-                                             _DT[x.dtype], _stream_ptr(x))
+            args = (x.data_ptr(), _ptr(res), g.data_ptr(), pd, mean.data_ptr(), rstd.data_ptr(), dy.data_ptr(),
+                    _ptr(dy2), ld2, dx.data_ptr(), _ptr(dres), dgb[0].data_ptr(), dgb[1].data_ptr())
+            tail = (rows, C, drop_p, seed, _ptr(ctx.sbase) if drop_p > 0.0 else 0, _DT[x.dtype], _stream_ptr(x))
+            if deterministic():
+                need = int(lib.bevf_layernorm_backward_workspace_bytes(rows, C))
+                ws = torch.empty(max(need, 16), device=x.device, dtype=torch.uint8)
+                st = lib.bevf_layernorm_backward_det(*args, ws.data_ptr(), need, *tail)
+            else:
+                st = lib.bevf_layernorm_backward(*args, *tail)
         _lib.check(st, lib)
         d_res = None if not has_res else (dres if dres is not None else dx)
         if ctx.arena is not None:
@@ -907,11 +1019,7 @@ def linear_wgrad_tc(dy, x, with_bias=False, out_dtype=None):
     buf = torch.zeros(N * K + (npad if with_bias else 0), device=x.device, dtype=torch.float32)
     dw = buf[: N * K].view(N, K)
     db = buf[N * K: N * K + N] if with_bias else None
-    lib = _lib.load()
-    with torch.cuda.device(x.device):
-        st = lib.bevf_linear_wgrad(dy.data_ptr(), x.data_ptr(), dw.data_ptr(), _ptr(db), M, N, K,
-                                   _stream_ptr(x))
-    _lib.check(st, lib)
+    _wgrad_acc(dy, x, dw, db)
     if out_dtype is not None and out_dtype != torch.float32:
         buf = buf.to(out_dtype)
         dw = buf[: N * K].view(N, K)
@@ -930,10 +1038,23 @@ def linear_wgrad_into(dy, x, dw_acc, db_acc=None):
     K = x.shape[1]
     if dw_acc.dtype != torch.float32 or dw_acc.numel() != N * K or not dw_acc.is_contiguous():
         raise RuntimeError("linear_wgrad_into: dw_acc must be a contiguous fp32 (N, K) buffer")
+    _wgrad_acc(dy, x, dw_acc, db_acc)
+
+
+def _wgrad_acc(dy, x, dw, db):
+    """dw += dy^T x (db += column sums of dy): split-M partial tiles reduced into dw with fp32 atomics, or -- in
+    deterministic mode -- stored into per-split slabs and summed in split order (bevf_linear_wgrad_into)."""
+    M, N = dy.shape
+    K = x.shape[1]
     lib = _lib.load()
     with torch.cuda.device(x.device):
-        st = lib.bevf_linear_wgrad(dy.data_ptr(), x.data_ptr(), dw_acc.data_ptr(), _ptr(db_acc), M, N, K,
-                                   _stream_ptr(x))
+        if deterministic() and M > 0:
+            need = int(lib.bevf_linear_wgrad_workspace_bytes(M, N, K))
+            ws = torch.empty(need, device=x.device, dtype=torch.uint8)
+            st = lib.bevf_linear_wgrad_into(dy.data_ptr(), x.data_ptr(), dw.data_ptr(), _ptr(db), ws.data_ptr(), need,
+                                            M, N, K, _stream_ptr(x))
+        else:
+            st = lib.bevf_linear_wgrad(dy.data_ptr(), x.data_ptr(), dw.data_ptr(), _ptr(db), M, N, K, _stream_ptr(x))
     _lib.check(st, lib)
 
 
@@ -985,7 +1106,13 @@ def colsum(x):
     out = torch.zeros(C, device=x.device, dtype=torch.float32)
     lib = _lib.load()
     with torch.cuda.device(x.device):
-        st = lib.bevf_colsum(x.data_ptr(), out.data_ptr(), rows, C, _DT[x.dtype], _stream_ptr(x))
+        if deterministic() and rows > 0:
+            need = int(lib.bevf_colsum_workspace_bytes(rows, C))
+            ws = torch.empty(need, device=x.device, dtype=torch.uint8)
+            st = lib.bevf_colsum_det(x.data_ptr(), out.data_ptr(), ws.data_ptr(), need, rows, C, _DT[x.dtype],
+                                     _stream_ptr(x))
+        else:
+            st = lib.bevf_colsum(x.data_ptr(), out.data_ptr(), rows, C, _DT[x.dtype], _stream_ptr(x))
     _lib.check(st, lib)
     return out
 

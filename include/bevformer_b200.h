@@ -90,7 +90,8 @@ BEVF_API int bevf_msda_forward(const void *value, int value_dtype, const int64_t
  *                                   multi_scale_deformable_attn_function.py:146)
  *   grad_loc    (B, Q, M, L, P, 2) f32 -- fully overwritten (zeros for skipped samples)
  *   grad_attn   (B, Q, M, L, P)    f32 -- fully overwritten
- * grad_value uses vector fp32 reductions in L2; its summation order is not deterministic.
+ * grad_value uses vector fp32 reductions in L2; its summation order is not deterministic
+ * (bevf_msda_backward_fx below is the deterministic form).
  */
 BEVF_API int bevf_msda_backward(const void *value, int value_dtype, const int64_t *level_hw,
                        const int64_t *level_start, const float *loc, const float *attn,
@@ -178,6 +179,45 @@ BEVF_API int bevf_msda_rows_backward_mixed(const void *value, int value_dtype, c
                                            int B, int S, int M, int D, int R, int L, int P, void *stream);
 BEVF_API int bevf_gv_merge(const void *fine_f16, const float *side_f32, const uint32_t *amax_bits, void *out_bf16,
                            int B, int S, int S_fine, int row_elems, void *stream);
+
+/*
+ * DETERMINISTIC sampler backward: grad_value summed in 64-bit fixed point.  Integer addition is associative, so the
+ * result does not depend on the order in which the samples are processed (any row order, any schedule gives the same
+ * bits).  grad_loc / grad_attn are those of bevf_msda_backward / bevf_msda_rows_backward bit for bit.
+ *
+ *   bevf_msda_fx_frac_bits(rows_per_map, L, P)   the fraction bits K for a launch: min(40, 62 - ceil(log2(n_max)))
+ *                                                with n_max = rows_per_map * L * P * 4, the most contributions one
+ *                                                element can receive (rows_per_map = Q, or R for a row list);
+ *                                                n_max * 2^K <= 2^62, so the sum cannot overflow.  -1 if no K fits.
+ *   bevf_msda_backward_fx / _rows_backward_fx    arguments as bevf_msda_backward / bevf_msda_rows_backward, plus
+ *       grad_value_fx  (B, S, M, D) int64 -- ACCUMULATED INTO (caller zero-fills)
+ *       bounds         2 uint32 DEVICE words, written: the bits of max|attn| and max|grad_out| over the launch's rows
+ *                      (rows with row_map < 0 excluded), sign cleared; the conversion reads them
+ *       frac_bits      K, at most bevf_msda_fx_frac_bits(Q or R, L, P)
+ *   bevf_msda_fx_convert(fx, bounds, K, out, out_dtype, accumulate, n)   out (f32 | bf16) = fx * 2^(E - K), or
+ *                                                out += that with accumulate != 0 (bevf_msda_backward's contract)
+ * Scale: E = (floor(log2 max|attn|) + 1) + (floor(log2 max|grad_out|) + 1), so every contribution w * attn * g
+ * (w <= 1) is below 2^E.  A contribution is formed exactly (the fp32 products w * attn and (w * attn) * g in double),
+ * scaled by 2^(K - E) and rounded to the nearest integer once.  PRECISION: an element that receives n contributions
+ * differs from their exact sum by at most n * 2^(E - K - 1) before the final rounding to out_dtype (with K = 40:
+ * n * 2^-39 of 4 * max|attn| * max|grad_out|).
+ * NON-FINITE INPUT: if attn or grad_out holds an inf or NaN in a live row, nothing is accumulated and the conversion
+ * makes every element of grad_value NaN (with accumulate: NaN is added).
+ */
+BEVF_API int bevf_msda_fx_frac_bits(int64_t rows_per_map, int L, int P);
+BEVF_API int bevf_msda_backward_fx(const void *value, int value_dtype, const int64_t *level_hw,
+                                   const int64_t *level_start, const float *loc, const float *attn,
+                                   const void *grad_out, int grad_out_dtype, int64_t *grad_value_fx, uint32_t *bounds,
+                                   int frac_bits, float *grad_loc, float *grad_attn, int B, int S, int M, int D, int Q,
+                                   int L, int P, void *stream);
+BEVF_API int bevf_msda_rows_backward_fx(const void *value, int value_dtype, const int64_t *level_hw,
+                                        const int64_t *level_start, const float *loc, const float *attn,
+                                        const void *grad_out, int grad_out_dtype, int64_t *grad_value_fx,
+                                        uint32_t *bounds, int frac_bits, float *grad_loc, float *grad_attn,
+                                        const int32_t *row_map, int B, int S, int M, int D, int R, int L, int P,
+                                        void *stream);
+BEVF_API int bevf_msda_fx_convert(const int64_t *grad_value_fx, const uint32_t *bounds, int frac_bits, void *out,
+                                  int out_dtype, int accumulate, int64_t n, void *stream);
 
 /*
  * bevf_msda_rows_forward with the coarse pyramid levels staged in shared memory by TMA.
@@ -343,6 +383,18 @@ BEVF_API int bevf_layernorm_backward(const void *x, const void *residual, const 
                                      int C, float drop_p, uint64_t seed, const uint64_t *seed_base,
                                      int dtype, void *stream);
 
+/* Deterministic form of bevf_layernorm_backward: the warps of a CTA are combined in index order and every CTA stores
+ * its [dgamma | dbeta] partial row into `workspace`; a second kernel sums the rows in CTA order and adds them into
+ * dgamma / dbeta (still ACCUMULATED INTO).  Same results run to run on one GPU model (the partition follows the SM
+ * count).  bevf_layernorm_backward_workspace_bytes(rows, C) gives the workspace size. */
+BEVF_API int64_t bevf_layernorm_backward_workspace_bytes(int64_t rows, int C);
+BEVF_API int bevf_layernorm_backward_det(const void *x, const void *residual, const void *gamma,
+                                         int param_dtype, const float *mean, const float *rstd,
+                                         const void *dy, const void *dy_plus_pos, int64_t dy_plus_pos_ld,
+                                         void *dx, void *dres, float *dgamma, float *dbeta, void *workspace,
+                                         int64_t workspace_bytes, int64_t rows, int C, float drop_p, uint64_t seed,
+                                         const uint64_t *seed_base, int dtype, void *stream);
+
 /*
  * slots[b,q,:] = inv_count[b,q] * sum_{cameras seeing q} out[b*R + pair_of[cam][q], :]
  * replaces spatial_cross_attention.py:165-172 (python scatter-add loops, count, divide).
@@ -430,6 +482,12 @@ BEVF_API int bevf_sum_tensors(const void *const *srcs, int n, void *out, int64_t
 
 BEVF_API int bevf_colsum(const void *x, float *out, int64_t rows, int C, int dtype, void *stream);
 
+/* Deterministic form of bevf_colsum: per-CTA column sums stored into `workspace`, then summed in CTA order and added
+ * into out.  bevf_colsum_workspace_bytes(rows, C) gives the workspace size. */
+BEVF_API int64_t bevf_colsum_workspace_bytes(int64_t rows, int C);
+BEVF_API int bevf_colsum_det(const void *x, float *out, void *workspace, int64_t workspace_bytes, int64_t rows, int C,
+                             int dtype, void *stream);
+
 /*
  * The FFN's hidden dropout (mmcv FFN: Linear -> ReLU -> Dropout; the ReLU itself is fused into
  * bevf_linear_forward's epilogue) and the joint backward of dropout(relu(z)).
@@ -455,6 +513,11 @@ BEVF_API int64_t bevf_linear_wgrad_workspace_bytes(int64_t M, int N, int K);
 BEVF_API int bevf_linear_wgrad_out(const void *dy, const void *x, void *dw, void *db, int grad_dtype,
                                    void *workspace, int64_t workspace_bytes, int64_t M, int N, int K,
                                    void *stream);
+/* The same two passes, ACCUMULATING into fp32 dw (N, K) / db (N) (the gradient arena).  Both passes sum in a fixed
+ * order (the bias column sums of pass 1 too), so this and bevf_linear_wgrad_out are deterministic run to run on one
+ * GPU model; the workspace is bevf_linear_wgrad_workspace_bytes(M, N, K). */
+BEVF_API int bevf_linear_wgrad_into(const void *dy, const void *x, float *dw, float *db, void *workspace,
+                                    int64_t workspace_bytes, int64_t M, int N, int K, void *stream);
 
 #ifdef __cplusplus
 }

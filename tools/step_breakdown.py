@@ -2,7 +2,7 @@
 
 Runs the same step as bench.py eagerly under torch.profiler (CUPTI activity records: real kernel
 durations, warm caches, no replay) and prints the kernels grouped by name with their time per step.
-Usage: python tools/step_breakdown.py [--steps 2] [--out gpurun_out/step_breakdown.txt]
+Usage: python tools/step_breakdown.py [--steps 2] [--deterministic] [--out results/step_breakdown.txt]
 """
 from __future__ import annotations
 
@@ -13,6 +13,7 @@ import re
 import sys
 
 import torch
+import torch.utils.deterministic
 
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 from bevformer_b200 import synthetic as syn  # noqa: E402
@@ -31,7 +32,13 @@ def main():
     ap.add_argument("--steps", type=int, default=2)
     ap.add_argument("--workload", default="base")
     ap.add_argument("--out", default=None)
+    ap.add_argument("--deterministic", action="store_true",
+                    help="torch.use_deterministic_algorithms(True) (uninitialised-memory fill off)")
     args = ap.parse_args()
+    if args.deterministic:
+        os.environ.setdefault("CUBLAS_WORKSPACE_CONFIG", ":4096:8")
+        torch.use_deterministic_algorithms(True)
+        torch.utils.deterministic.fill_uninitialized_memory = False
     dev = torch.device("cuda", 0)
     w = syn.WORKLOADS[args.workload]
     dtype = torch.bfloat16
