@@ -89,6 +89,14 @@ SIGNATURES = {
                                                       c_void_p]),
     "bevf_sum_tensors": (c_int, [c_void_p, c_int, c_void_p, c_int64, c_int, c_void_p]),
     "bevf_linear_wgrad_into": (c_int, [c_void_p] * 5 + [c_int64, c_int64, c_int, c_int, c_void_p]),
+    "bevf_linear_forward_dt": (c_int, [c_void_p] * 3 + [c_int] + [c_void_p] * 2
+                               + [c_int, c_int64, c_int, c_int, c_int, c_int, c_void_p]),
+    "bevf_linear_dgrad_dt": (c_int, [c_void_p] * 3 + [c_int64, c_int, c_int, c_int, c_void_p]),
+    "bevf_linear_dgrad_acc_dt": (c_int, [c_void_p] * 4 + [c_int64, c_int, c_int, c_int, c_void_p]),
+    "bevf_linear_wgrad_dt": (c_int, [c_void_p] * 4 + [c_int64, c_int, c_int, c_int, c_void_p]),
+    "bevf_linear_wgrad_out_dt": (c_int, [c_void_p] * 4 + [c_int, c_void_p, c_int64, c_int64, c_int, c_int, c_int,
+                                                         c_void_p]),
+    "bevf_linear_wgrad_into_dt": (c_int, [c_void_p] * 5 + [c_int64, c_int64, c_int, c_int, c_int, c_void_p]),
     "bevf_colsum": (c_int, [c_void_p, c_void_p, c_int64, c_int, c_int, c_void_p]),
     "bevf_colsum_workspace_bytes": (c_int64, [c_int64, c_int]),
     "bevf_colsum_det": (c_int, [c_void_p, c_void_p, c_void_p, c_int64, c_int64, c_int, c_int, c_void_p]),

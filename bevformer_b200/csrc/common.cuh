@@ -2,6 +2,7 @@
 #pragma once
 
 #include <cuda_bf16.h>
+#include <cuda_fp16.h>
 #include <cuda_runtime.h>
 #include <stdint.h>
 
@@ -72,6 +73,34 @@ __device__ __forceinline__ uint32_t pack_bf16x2(float lo, float hi) {
     return r;
 }
 
+// fp16 storage: widening is exact; stores round to nearest and overflow to +-inf (no saturation: loss scaling
+// detects overflow through the inf / NaN it leaves behind)
+__device__ __forceinline__ float f16_lo(uint32_t u) { return __half2float(__ushort_as_half((unsigned short)(u & 0xffffu))); }
+__device__ __forceinline__ float f16_hi(uint32_t u) { return __half2float(__ushort_as_half((unsigned short)(u >> 16))); }
+__device__ __forceinline__ uint32_t pack_f16x2(float lo, float hi) {
+    // cvt.rn.f16x2.f32 d, a, b  puts a in the upper half, b in the lower half
+    uint32_t r;
+    asm("cvt.rn.f16x2.f32 %0, %1, %2;" : "=r"(r) : "f"(hi), "f"(lo));
+    return r;
+}
+
+// The two 16-bit storage types behind one interface: halves of a 32-bit word <-> fp32.
+template <typename T> struct St16;
+template <> struct St16<bf16> {
+    __device__ static __forceinline__ float lo(uint32_t u) { return bf16_lo(u); }
+    __device__ static __forceinline__ float hi(uint32_t u) { return bf16_hi(u); }
+    __device__ static __forceinline__ uint32_t pack(float lo, float hi) { return pack_bf16x2(lo, hi); }
+    __device__ static __forceinline__ float to_f(bf16 v) { return __bfloat162float(v); }
+    __device__ static __forceinline__ bf16 from_f(float v) { return __float2bfloat16_rn(v); }
+};
+template <> struct St16<__half> {
+    __device__ static __forceinline__ float lo(uint32_t u) { return f16_lo(u); }
+    __device__ static __forceinline__ float hi(uint32_t u) { return f16_hi(u); }
+    __device__ static __forceinline__ uint32_t pack(float lo, float hi) { return pack_f16x2(lo, hi); }
+    __device__ static __forceinline__ float to_f(__half v) { return __half2float(v); }
+    __device__ static __forceinline__ __half from_f(float v) { return __float2half_rn(v); }
+};
+
 // A "row" is the 32 contiguous channels of one (pixel, head).  kVec channels per lane, 16 B each.
 template <typename T> struct Row;
 template <> struct Row<float> {
@@ -86,55 +115,51 @@ template <> struct Row<float> {
     __device__ static __forceinline__ float load1(const float *p) { return __ldg(p); }
     __device__ static __forceinline__ void store1(float *p, float v) { *p = v; }
 };
-template <> struct Row<bf16> {
+// bf16 / fp16: kVec = 8
+template <typename T> struct Row {
     static constexpr int kVec = 8;
-    __device__ static __forceinline__ void load(const bf16 *p, float (&v)[8]) {
+    __device__ static __forceinline__ void load(const T *p, float (&v)[8]) {
         uint4 t = __ldg(reinterpret_cast<const uint4 *>(p));
-        v[0] = bf16_lo(t.x); v[1] = bf16_hi(t.x); v[2] = bf16_lo(t.y); v[3] = bf16_hi(t.y);
-        v[4] = bf16_lo(t.z); v[5] = bf16_hi(t.z); v[6] = bf16_lo(t.w); v[7] = bf16_hi(t.w);
+        v[0] = St16<T>::lo(t.x); v[1] = St16<T>::hi(t.x); v[2] = St16<T>::lo(t.y); v[3] = St16<T>::hi(t.y);
+        v[4] = St16<T>::lo(t.z); v[5] = St16<T>::hi(t.z); v[6] = St16<T>::lo(t.w); v[7] = St16<T>::hi(t.w);
     }
-    __device__ static __forceinline__ void store(bf16 *p, const float (&v)[8]) {
+    __device__ static __forceinline__ void store(T *p, const float (&v)[8]) {
         uint4 t;
-        t.x = pack_bf16x2(v[0], v[1]); t.y = pack_bf16x2(v[2], v[3]);
-        t.z = pack_bf16x2(v[4], v[5]); t.w = pack_bf16x2(v[6], v[7]);
+        t.x = St16<T>::pack(v[0], v[1]); t.y = St16<T>::pack(v[2], v[3]);
+        t.z = St16<T>::pack(v[4], v[5]); t.w = St16<T>::pack(v[6], v[7]);
         *reinterpret_cast<uint4 *>(p) = t;
     }
-    __device__ static __forceinline__ float load1(const bf16 *p) {
-        return __bfloat162float(*p);
-    }
-    __device__ static __forceinline__ void store1(bf16 *p, float v) { *p = __float2bfloat16_rn(v); }
+    __device__ static __forceinline__ float load1(const T *p) { return St16<T>::to_f(*p); }
+    __device__ static __forceinline__ void store1(T *p, float v) { *p = St16<T>::from_f(v); }
 };
 
-// N consecutive channels (N = 4 or 8) <-> fp32 registers, for either storage type.
-template <typename T, int N> __device__ __forceinline__ void load_vec(const T *p, float (&v)[N]);
-template <> __device__ __forceinline__ void load_vec<float, 4>(const float *p, float (&v)[4]) {
-    Row<float>::load(p, v);
+// N consecutive channels (N = 4 or 8) <-> fp32 registers, for any storage type.
+template <typename T, int N> __device__ __forceinline__ void load_vec(const T *p, float (&v)[N]) {
+    static_assert(N == 4 || N == 8, "4 or 8 channels");
+    if constexpr (sizeof(T) == 4) {
+        const float4 a = __ldg(reinterpret_cast<const float4 *>(p));
+        v[0] = a.x; v[1] = a.y; v[2] = a.z; v[3] = a.w;
+        if constexpr (N == 8) {
+            const float4 b = __ldg(reinterpret_cast<const float4 *>(p) + 1);
+            v[4] = b.x; v[5] = b.y; v[6] = b.z; v[7] = b.w;
+        }
+    } else if constexpr (N == 8) {
+        Row<T>::load(p, v);
+    } else {
+        const uint2 t = __ldg(reinterpret_cast<const uint2 *>(p));
+        v[0] = St16<T>::lo(t.x); v[1] = St16<T>::hi(t.x); v[2] = St16<T>::lo(t.y); v[3] = St16<T>::hi(t.y);
+    }
 }
-template <> __device__ __forceinline__ void load_vec<float, 8>(const float *p, float (&v)[8]) {
-    const float4 a = __ldg(reinterpret_cast<const float4 *>(p));
-    const float4 b = __ldg(reinterpret_cast<const float4 *>(p) + 1);
-    v[0] = a.x; v[1] = a.y; v[2] = a.z; v[3] = a.w; v[4] = b.x; v[5] = b.y; v[6] = b.z; v[7] = b.w;
-}
-template <> __device__ __forceinline__ void load_vec<bf16, 8>(const bf16 *p, float (&v)[8]) {
-    Row<bf16>::load(p, v);
-}
-template <> __device__ __forceinline__ void load_vec<bf16, 4>(const bf16 *p, float (&v)[4]) {
-    const uint2 t = __ldg(reinterpret_cast<const uint2 *>(p));
-    v[0] = bf16_lo(t.x); v[1] = bf16_hi(t.x); v[2] = bf16_lo(t.y); v[3] = bf16_hi(t.y);
-}
-template <typename T, int N> __device__ __forceinline__ void store_vec(T *p, const float (&v)[N]);
-template <> __device__ __forceinline__ void store_vec<float, 4>(float *p, const float (&v)[4]) {
-    Row<float>::store(p, v);
-}
-template <> __device__ __forceinline__ void store_vec<float, 8>(float *p, const float (&v)[8]) {
-    reinterpret_cast<float4 *>(p)[0] = make_float4(v[0], v[1], v[2], v[3]);
-    reinterpret_cast<float4 *>(p)[1] = make_float4(v[4], v[5], v[6], v[7]);
-}
-template <> __device__ __forceinline__ void store_vec<bf16, 8>(bf16 *p, const float (&v)[8]) {
-    Row<bf16>::store(p, v);
-}
-template <> __device__ __forceinline__ void store_vec<bf16, 4>(bf16 *p, const float (&v)[4]) {
-    *reinterpret_cast<uint2 *>(p) = make_uint2(pack_bf16x2(v[0], v[1]), pack_bf16x2(v[2], v[3]));
+template <typename T, int N> __device__ __forceinline__ void store_vec(T *p, const float (&v)[N]) {
+    static_assert(N == 4 || N == 8, "4 or 8 channels");
+    if constexpr (sizeof(T) == 4) {
+        reinterpret_cast<float4 *>(p)[0] = make_float4(v[0], v[1], v[2], v[3]);
+        if constexpr (N == 8) reinterpret_cast<float4 *>(p)[1] = make_float4(v[4], v[5], v[6], v[7]);
+    } else if constexpr (N == 8) {
+        Row<T>::store(p, v);
+    } else {
+        *reinterpret_cast<uint2 *>(p) = make_uint2(St16<T>::pack(v[0], v[1]), St16<T>::pack(v[2], v[3]));
+    }
 }
 
 // 16-byte fp32 vector reduction into global memory (SASS: REDG.E.ADD.F32x4).
@@ -148,11 +173,6 @@ __device__ __forceinline__ void red_add_v4(float *p, float a, float b, float c, 
 __device__ __forceinline__ void red_add_v4_f16x2(void *p, uint32_t a, uint32_t b, uint32_t c, uint32_t d) {
     asm volatile("red.global.add.noftz.v4.f16x2 [%0], {%1, %2, %3, %4};"
                  :: "l"(p), "r"(a), "r"(b), "r"(c), "r"(d) : "memory");
-}
-__device__ __forceinline__ uint32_t pack_f16x2(float lo, float hi) {
-    uint32_t r;
-    asm("cvt.rn.f16x2.f32 %0, %1, %2;" : "=r"(r) : "f"(hi), "f"(lo));
-    return r;
 }
 // Power-of-two scale that puts max|grad_out| into [8, 16): sums of up to ~4000 unit-weight contributions stay below
 // fp16's 65504 and everything down to 2^-17 of the maximum stays a NORMAL fp16 number.  amax_bits = the float bits

@@ -59,11 +59,13 @@ sca_prep_fwd(const float *__restrict__ raw, const float *__restrict__ ref_cam,
     }
 }
 
-// scalar / pair stores into an f32 or bf16 gradient tensor
+// scalar / pair stores into an f32, bf16 or fp16 gradient tensor
 __device__ __forceinline__ void st1(float *p, float v) { *p = v; }
-__device__ __forceinline__ void st1(bf16 *p, float v) { *p = __float2bfloat16_rn(v); }
+template <typename T> __device__ __forceinline__ void st1(T *p, float v) { *p = St16<T>::from_f(v); }
 __device__ __forceinline__ void st2(float *p, float a, float b) { *reinterpret_cast<float2 *>(p) = make_float2(a, b); }
-__device__ __forceinline__ void st2(bf16 *p, float a, float b) { *reinterpret_cast<uint32_t *>(p) = pack_bf16x2(a, b); }
+template <typename T> __device__ __forceinline__ void st2(T *p, float a, float b) {
+    *reinterpret_cast<uint32_t *>(p) = St16<T>::pack(a, b);
+}
 
 // d_raw for every query: sums over the cameras that see it (pair_of[cam][q] = row or -1)
 template <typename TO>
@@ -164,24 +166,24 @@ template <int N> __device__ __forceinline__ void stv(float *p, const float (&v)[
     }
 }
 
-// d_raw may be wanted in bf16 (it feeds the bf16 dX / dW GEMMs of the offsets|logits head): the
+// d_raw may be wanted in bf16 / fp16 (it feeds the 16-bit dX / dW GEMMs of the offsets|logits head): the
 // rounding then happens here instead of in a separate cast pass over the tensor
-template <int N> __device__ __forceinline__ void stv(bf16 *p, const float (&v)[N]) {
+template <int N, typename T> __device__ __forceinline__ void stv(T *p, const float (&v)[N]) {
     if constexpr (N % 8 == 0) {
 #pragma unroll
         for (int i = 0; i < N; i += 8)
-            *reinterpret_cast<uint4 *>(p + i) = make_uint4(pack_bf16x2(v[i], v[i + 1]), pack_bf16x2(v[i + 2], v[i + 3]),
-                                                           pack_bf16x2(v[i + 4], v[i + 5]), pack_bf16x2(v[i + 6], v[i + 7]));
+            *reinterpret_cast<uint4 *>(p + i) = make_uint4(St16<T>::pack(v[i], v[i + 1]), St16<T>::pack(v[i + 2], v[i + 3]),
+                                                           St16<T>::pack(v[i + 4], v[i + 5]), St16<T>::pack(v[i + 6], v[i + 7]));
     } else if constexpr (N % 4 == 0) {
 #pragma unroll
         for (int i = 0; i < N; i += 4)
-            *reinterpret_cast<uint2 *>(p + i) = make_uint2(pack_bf16x2(v[i], v[i + 1]), pack_bf16x2(v[i + 2], v[i + 3]));
+            *reinterpret_cast<uint2 *>(p + i) = make_uint2(St16<T>::pack(v[i], v[i + 1]), St16<T>::pack(v[i + 2], v[i + 3]));
     } else if constexpr (N % 2 == 0) {
 #pragma unroll
-        for (int i = 0; i < N; i += 2) *reinterpret_cast<uint32_t *>(p + i) = pack_bf16x2(v[i], v[i + 1]);
+        for (int i = 0; i < N; i += 2) *reinterpret_cast<uint32_t *>(p + i) = St16<T>::pack(v[i], v[i + 1]);
     } else {
 #pragma unroll
-        for (int i = 0; i < N; ++i) p[i] = __float2bfloat16_rn(v[i]);
+        for (int i = 0; i < N; ++i) p[i] = St16<T>::from_f(v[i]);
     }
 }
 
@@ -500,7 +502,7 @@ template <typename T, int PER> struct RawRow {
             if constexpr (sizeof(T) == 2) {
                 const uint32_t u[4] = {q[ci].x, q[ci].y, q[ci].z, q[ci].w};
 #pragma unroll
-                for (int k = 0; k < 4; ++k) { v[ci * 8 + 2 * k] = bf16_lo(u[k]); v[ci * 8 + 2 * k + 1] = bf16_hi(u[k]); }
+                for (int k = 0; k < 4; ++k) { v[ci * 8 + 2 * k] = St16<T>::lo(u[k]); v[ci * 8 + 2 * k + 1] = St16<T>::hi(u[k]); }
             } else {
                 v[ci * 4] = __uint_as_float(q[ci].x); v[ci * 4 + 1] = __uint_as_float(q[ci].y);
                 v[ci * 4 + 2] = __uint_as_float(q[ci].z); v[ci * 4 + 3] = __uint_as_float(q[ci].w);
@@ -512,6 +514,7 @@ template <typename T, int PER> struct RawRow {
 template <typename TP> __device__ __forceinline__ float ldp(const TP *p, int i);
 template <> __device__ __forceinline__ float ldp<float>(const float *p, int i) { return __ldg(p + i); }
 template <> __device__ __forceinline__ float ldp<bf16>(const bf16 *p, int i) { return __bfloat162float(p[i]); }
+template <> __device__ __forceinline__ float ldp<__half>(const __half *p, int i) { return __half2float(p[i]); }
 
 constexpr int kLnRowsPerWarp = 4;
 
@@ -915,12 +918,15 @@ tsa_prep_m8(const float *__restrict__ raw, const float *__restrict__ ref2d,
 template <typename T> __device__ __forceinline__ float round_to(float v);
 template <> __device__ __forceinline__ float round_to<float>(float v) { return v; }
 template <> __device__ __forceinline__ float round_to<bf16>(float v) { return __bfloat162float(__float2bfloat16_rn(v)); }
+template <> __device__ __forceinline__ float round_to<__half>(float v) { return __half2float(__float2half_rn(v)); }
 template <typename T> __device__ __forceinline__ float to_f(T v);
 template <> __device__ __forceinline__ float to_f<float>(float v) { return v; }
 template <> __device__ __forceinline__ float to_f<bf16>(bf16 v) { return __bfloat162float(v); }
+template <> __device__ __forceinline__ float to_f<__half>(__half v) { return __half2float(v); }
 template <typename T> __device__ __forceinline__ T from_f(float v);
 template <> __device__ __forceinline__ float from_f<float>(float v) { return v; }
 template <> __device__ __forceinline__ bf16 from_f<bf16>(float v) { return __float2bfloat16_rn(v); }
+template <> __device__ __forceinline__ __half from_f<__half>(float v) { return __float2half_rn(v); }
 
 template <typename T>
 __global__ void __launch_bounds__(256)
@@ -1041,12 +1047,14 @@ extern "C" int bevf_sca_prep_backward(const float *raw, const float *grad_loc,
                                       int R, int M, int L, int P, int ncam, void *stream) {
     const char *who = "bevf_sca_prep_backward";
     BEVF_REQUIRE(B >= 0 && Nq >= 0 && R >= 0 && M > 0 && L > 0 && P > 0 && ncam > 0 && ncam <= 16, who, "bad dimension (ncam <= 16)");
-    BEVF_REQUIRE(out_dtype == BEVF_DTYPE_F32 || out_dtype == BEVF_DTYPE_BF16, who, "unsupported dtype code");
+    BEVF_REQUIRE(out_dtype == BEVF_DTYPE_F32 || out_dtype == BEVF_DTYPE_BF16 || out_dtype == BEVF_DTYPE_F16, who, "unsupported dtype code");
     if ((long long)B * Nq * M == 0) return 0;
     BEVF_REQUIRE(raw && pair_of && level_hw && d_raw && (R == 0 || (grad_loc && grad_attn)), who, "null pointer argument");
     cudaStream_t st = (cudaStream_t)stream;
     if (out_dtype == BEVF_DTYPE_BF16)
         return sca_prep_backward_t<bf16>(who, raw, grad_loc, grad_attn, pair_of, level_hw, (bf16 *)d_raw, B, Nq, R, M, L, P, ncam, st);
+    if (out_dtype == BEVF_DTYPE_F16)
+        return sca_prep_backward_t<__half>(who, raw, grad_loc, grad_attn, pair_of, level_hw, (__half *)d_raw, B, Nq, R, M, L, P, ncam, st);
     return sca_prep_backward_t<float>(who, raw, grad_loc, grad_attn, pair_of, level_hw, (float *)d_raw, B, Nq, R, M, L, P, ncam, st);
 }
 
@@ -1087,12 +1095,14 @@ extern "C" int bevf_tsa_prep_backward(const float *raw, const float *grad_loc,
                                       void *stream) {
     const char *who = "bevf_tsa_prep_backward";
     BEVF_REQUIRE(B >= 0 && Nq >= 0 && M > 0 && L > 0 && P > 0, who, "bad dimension");
-    BEVF_REQUIRE(out_dtype == BEVF_DTYPE_F32 || out_dtype == BEVF_DTYPE_BF16, who, "unsupported dtype code");
+    BEVF_REQUIRE(out_dtype == BEVF_DTYPE_F32 || out_dtype == BEVF_DTYPE_BF16 || out_dtype == BEVF_DTYPE_F16, who, "unsupported dtype code");
     if ((long long)B * Nq * M * 2 == 0) return 0;
     BEVF_REQUIRE(raw && grad_loc && grad_attn && level_hw && d_raw, who, "null pointer argument");
     cudaStream_t st = (cudaStream_t)stream;
     if (out_dtype == BEVF_DTYPE_BF16)
         return tsa_prep_backward_t<bf16>(who, raw, grad_loc, grad_attn, level_hw, (bf16 *)d_raw, B, Nq, M, L, P, interleave, st);
+    if (out_dtype == BEVF_DTYPE_F16)
+        return tsa_prep_backward_t<__half>(who, raw, grad_loc, grad_attn, level_hw, (__half *)d_raw, B, Nq, M, L, P, interleave, st);
     return tsa_prep_backward_t<float>(who, raw, grad_loc, grad_attn, level_hw, (float *)d_raw, B, Nq, M, L, P, interleave, st);
 }
 
@@ -1125,7 +1135,13 @@ extern "C" int bevf_layernorm_forward(const void *x, const void *residual, const
     BEVF_REQUIRE(drop_p >= 0.f && drop_p < 1.f, who, "dropout probability must be in [0, 1)");
     cudaStream_t st = (cudaStream_t)stream;
     const bool pb = param_dtype == BEVF_DTYPE_BF16;
-    BEVF_REQUIRE(pb || param_dtype == BEVF_DTYPE_F32, who, "unsupported parameter dtype code");
+    BEVF_REQUIRE(pb || param_dtype == BEVF_DTYPE_F32 || param_dtype == BEVF_DTYPE_F16, who, "unsupported parameter dtype code");
+    if (dtype == BEVF_DTYPE_F16) {
+        if (pb) return fail("%s: bf16 parameters with fp16 activations are not supported", who);
+        if (param_dtype == BEVF_DTYPE_F16) return ln_fwd_t<__half, __half>(who, x, residual, gamma, beta, pos, y, y_plus_pos, mean, rstd, rows, C, eps, drop_p, seed, sb, st);
+        return ln_fwd_t<__half, float>(who, x, residual, gamma, beta, pos, y, y_plus_pos, mean, rstd, rows, C, eps, drop_p, seed, sb, st);
+    }
+    if (param_dtype == BEVF_DTYPE_F16) return fail("%s: fp16 parameters need fp16 activations", who);
     if (dtype == BEVF_DTYPE_F32) {
         if (pb) return fail("%s: bf16 parameters with fp32 activations are not supported", who);
         return ln_fwd_t<float, float>(who, x, residual, gamma, beta, pos, y, y_plus_pos, mean, rstd, rows, C, eps, drop_p, seed, sb, st);
@@ -1178,11 +1194,17 @@ static int layernorm_backward_impl(const char *who, const void *x, const void *r
     if (rows == 0) return 0;
     BEVF_REQUIRE(x && gamma && mean && rstd && dy && dx && dgamma && dbeta, who, "null pointer argument");
     const long long ld2 = dy_plus_pos_ld > 0 ? (long long)dy_plus_pos_ld : (long long)C;
-    BEVF_REQUIRE(ld2 >= C && ld2 % (dtype == BEVF_DTYPE_BF16 ? 8 : 4) == 0, who, "bad row stride of dy_plus_pos");
+    BEVF_REQUIRE(ld2 >= C && ld2 % (dtype != BEVF_DTYPE_F32 ? 8 : 4) == 0, who, "bad row stride of dy_plus_pos");
     BEVF_REQUIRE(drop_p == 0.f || dres != nullptr || residual == nullptr, who, "dropout with a residual needs a separate dres buffer");
     cudaStream_t st = (cudaStream_t)stream;
     const bool pb = param_dtype == BEVF_DTYPE_BF16;
-    BEVF_REQUIRE(pb || param_dtype == BEVF_DTYPE_F32, who, "unsupported parameter dtype code");
+    BEVF_REQUIRE(pb || param_dtype == BEVF_DTYPE_F32 || param_dtype == BEVF_DTYPE_F16, who, "unsupported parameter dtype code");
+    if (dtype == BEVF_DTYPE_F16) {
+        if (pb) return fail("%s: bf16 parameters with fp16 activations are not supported", who);
+        if (param_dtype == BEVF_DTYPE_F16) return ln_bwd_t<__half, __half>(who, x, residual, gamma, mean, rstd, dy, dy_plus_pos, dx, dres, dgamma, dbeta, rows, C, drop_p, seed, sb, ld2, st, part);
+        return ln_bwd_t<__half, float>(who, x, residual, gamma, mean, rstd, dy, dy_plus_pos, dx, dres, dgamma, dbeta, rows, C, drop_p, seed, sb, ld2, st, part);
+    }
+    if (param_dtype == BEVF_DTYPE_F16) return fail("%s: fp16 parameters need fp16 activations", who);
     if (dtype == BEVF_DTYPE_F32) {
         if (pb) return fail("%s: bf16 parameters with fp32 activations are not supported", who);
         return ln_bwd_t<float, float>(who, x, residual, gamma, mean, rstd, dy, dy_plus_pos, dx, dres, dgamma, dbeta, rows, C, drop_p, seed, sb, ld2, st, part);
@@ -1242,6 +1264,8 @@ extern "C" int bevf_sca_combine_forward(const void *out, const int32_t *pair_of,
         sca_combine_fwd<float><<<blocks_for((long long)B * Nq * (C / 4), kEThreads), kEThreads, 0, st>>>((const float *)out, pair_of, inv_count, (float *)slots, B, Nq, R, C, ncam);
     } else if (dtype == BEVF_DTYPE_BF16) {
         sca_combine_fwd<bf16><<<blocks_for((long long)B * Nq * (C / 8), kEThreads), kEThreads, 0, st>>>((const bf16 *)out, pair_of, inv_count, (bf16 *)slots, B, Nq, R, C, ncam);
+    } else if (dtype == BEVF_DTYPE_F16) {
+        sca_combine_fwd<__half><<<blocks_for((long long)B * Nq * (C / 8), kEThreads), kEThreads, 0, st>>>((const __half *)out, pair_of, inv_count, (__half *)slots, B, Nq, R, C, ncam);
     } else {
         return fail("%s: unsupported dtype code", who);
     }
@@ -1260,6 +1284,8 @@ extern "C" int bevf_sca_combine_backward(const void *g_slots, const int32_t *pai
         sca_combine_bwd<float><<<blocks_for((long long)B * R * (C / 4), kEThreads), kEThreads, 0, st>>>((const float *)g_slots, pair_q, inv_count, (float *)g_out, B, Nq, R, C);
     } else if (dtype == BEVF_DTYPE_BF16) {
         sca_combine_bwd<bf16><<<blocks_for((long long)B * R * (C / 8), kEThreads), kEThreads, 0, st>>>((const bf16 *)g_slots, pair_q, inv_count, (bf16 *)g_out, B, Nq, R, C);
+    } else if (dtype == BEVF_DTYPE_F16) {
+        sca_combine_bwd<__half><<<blocks_for((long long)B * R * (C / 8), kEThreads), kEThreads, 0, st>>>((const __half *)g_slots, pair_q, inv_count, (__half *)g_out, B, Nq, R, C);
     } else {
         return fail("%s: unsupported dtype code", who);
     }
@@ -1299,6 +1325,8 @@ extern "C" int bevf_flatten_feats(const void *feat, const float *cams_embeds, co
         flatten_feats_kernel<float><<<grid, 256, 0, st>>>((const float *)feat, cams_embeds, level_embed, (float *)out, bs, ncam, C, hw, S, level_start);
     else if (dtype == BEVF_DTYPE_BF16)
         flatten_feats_kernel<bf16><<<grid, 256, 0, st>>>((const bf16 *)feat, cams_embeds, level_embed, (bf16 *)out, bs, ncam, C, hw, S, level_start);
+    else if (dtype == BEVF_DTYPE_F16)
+        flatten_feats_kernel<__half><<<grid, 256, 0, st>>>((const __half *)feat, cams_embeds, level_embed, (__half *)out, bs, ncam, C, hw, S, level_start);
     else
         return fail("%s: unsupported dtype code", who);
     return check_launch(who);
@@ -1330,8 +1358,8 @@ extern "C" int bevf_sum_tensors(const void *const *srcs, int n, void *out, int64
     BEVF_REQUIRE(n >= 1 && n <= 8 && numel >= 0, who, "1..8 tensors");
     if (numel == 0) return 0;
     BEVF_REQUIRE(srcs && out, who, "null pointer argument");
-    BEVF_REQUIRE(dtype == BEVF_DTYPE_BF16 || dtype == BEVF_DTYPE_F32, who, "unsupported dtype code");
-    const int vec = dtype == BEVF_DTYPE_BF16 ? 8 : 4;
+    BEVF_REQUIRE(dtype == BEVF_DTYPE_BF16 || dtype == BEVF_DTYPE_F16 || dtype == BEVF_DTYPE_F32, who, "unsupported dtype code");
+    const int vec = dtype != BEVF_DTYPE_F32 ? 8 : 4;
     BEVF_REQUIRE(numel % vec == 0, who, "numel must be a multiple of 16 bytes");
     SumPtrs sp;
     for (int k = 0; k < 8; ++k) {
@@ -1345,6 +1373,8 @@ extern "C" int bevf_sum_tensors(const void *const *srcs, int n, void *out, int64
     cudaStream_t st = (cudaStream_t)stream;
     if (dtype == BEVF_DTYPE_BF16)
         sum_n_kernel<bf16><<<(unsigned)blocks, kEThreads, 0, st>>>(sp, n, (bf16 *)out, vecs);
+    else if (dtype == BEVF_DTYPE_F16)
+        sum_n_kernel<__half><<<(unsigned)blocks, kEThreads, 0, st>>>(sp, n, (__half *)out, vecs);
     else
         sum_n_kernel<float><<<(unsigned)blocks, kEThreads, 0, st>>>(sp, n, (float *)out, vecs);
     return check_launch(who);
@@ -1361,8 +1391,8 @@ static int colsum_impl(const char *who, const void *x, float *out, int64_t rows,
     BEVF_REQUIRE(rows >= 0 && C > 0, who, "bad dimension");
     if (rows == 0) return 0;
     BEVF_REQUIRE(x && out, who, "null pointer argument");
-    const int vec = dtype == BEVF_DTYPE_BF16 ? 8 : 4;
-    BEVF_REQUIRE(dtype == BEVF_DTYPE_BF16 || dtype == BEVF_DTYPE_F32, who, "unsupported dtype code");
+    const int vec = dtype != BEVF_DTYPE_F32 ? 8 : 4;
+    BEVF_REQUIRE(dtype == BEVF_DTYPE_BF16 || dtype == BEVF_DTYPE_F16 || dtype == BEVF_DTYPE_F32, who, "unsupported dtype code");
     BEVF_REQUIRE(C % vec == 0 && C / vec <= kEThreads, who, "C must be a multiple of the vector width and <= 2048");
     long long rows_per_cta;
     const unsigned grid = colsum_plan(rows, rows_per_cta);
@@ -1371,6 +1401,8 @@ static int colsum_impl(const char *who, const void *x, float *out, int64_t rows,
     BEVF_REQUIRE(sm <= 48 * 1024, who, "C too large for the row-lane staging");
     if (dtype == BEVF_DTYPE_BF16)
         colsum_kernel<bf16><<<grid, kEThreads, sm, st>>>((const bf16 *)x, out, rows, C, (int)rows_per_cta, part);
+    else if (dtype == BEVF_DTYPE_F16)
+        colsum_kernel<__half><<<grid, kEThreads, sm, st>>>((const __half *)x, out, rows, C, (int)rows_per_cta, part);
     else
         colsum_kernel<float><<<grid, kEThreads, sm, st>>>((const float *)x, out, rows, C, (int)rows_per_cta, part);
     if (int e = check_launch(who)) return e;
@@ -1407,13 +1439,15 @@ extern "C" int bevf_relu_dropout_backward(const void *dy, const void *h, void *o
     BEVF_REQUIRE(n >= 0, who, "bad dimension");
     if (n == 0) return 0;
     BEVF_REQUIRE(dy && h && out, who, "null pointer argument");
-    const int vec = dtype == BEVF_DTYPE_BF16 ? 8 : 4;
-    BEVF_REQUIRE(dtype == BEVF_DTYPE_BF16 || dtype == BEVF_DTYPE_F32, who, "unsupported dtype code");
+    const int vec = dtype != BEVF_DTYPE_F32 ? 8 : 4;
+    BEVF_REQUIRE(dtype == BEVF_DTYPE_BF16 || dtype == BEVF_DTYPE_F16 || dtype == BEVF_DTYPE_F32, who, "unsupported dtype code");
     BEVF_REQUIRE(n % vec == 0, who, "element count must be a multiple of the vector width");
     const long long nv = n / vec;
     cudaStream_t st = (cudaStream_t)stream;
     if (dtype == BEVF_DTYPE_BF16)
         relu_dropout_bwd_kernel<bf16><<<blocks_for(nv, kEThreads), kEThreads, 0, st>>>((const bf16 *)dy, (const bf16 *)h, (bf16 *)out, nv, scale);
+    else if (dtype == BEVF_DTYPE_F16)
+        relu_dropout_bwd_kernel<__half><<<blocks_for(nv, kEThreads), kEThreads, 0, st>>>((const __half *)dy, (const __half *)h, (__half *)out, nv, scale);
     else
         relu_dropout_bwd_kernel<float><<<blocks_for(nv, kEThreads), kEThreads, 0, st>>>((const float *)dy, (const float *)h, (float *)out, nv, scale);
     return check_launch(who);
@@ -1426,14 +1460,16 @@ extern "C" int bevf_dropout_inplace(void *x, int64_t n, float p, uint64_t seed, 
     BEVF_REQUIRE(p >= 0.f && p < 1.f, who, "dropout probability must be in [0, 1)");
     if (n == 0 || p == 0.f) return 0;
     BEVF_REQUIRE(x, who, "null pointer argument");
-    const int vec = dtype == BEVF_DTYPE_BF16 ? 8 : 4;
-    BEVF_REQUIRE(dtype == BEVF_DTYPE_BF16 || dtype == BEVF_DTYPE_F32, who, "unsupported dtype code");
+    const int vec = dtype != BEVF_DTYPE_F32 ? 8 : 4;
+    BEVF_REQUIRE(dtype == BEVF_DTYPE_BF16 || dtype == BEVF_DTYPE_F16 || dtype == BEVF_DTYPE_F32, who, "unsupported dtype code");
     BEVF_REQUIRE(n % vec == 0, who, "element count must be a multiple of the vector width");
     const long long nv = n / vec;
     cudaStream_t st = (cudaStream_t)stream;
     const unsigned long long *sb = reinterpret_cast<const unsigned long long *>(seed_base);
     if (dtype == BEVF_DTYPE_BF16)
         dropout_inplace_kernel<bf16><<<blocks_for(nv, kEThreads), kEThreads, 0, st>>>((bf16 *)x, nv, p, seed, sb);
+    else if (dtype == BEVF_DTYPE_F16)
+        dropout_inplace_kernel<__half><<<blocks_for(nv, kEThreads), kEThreads, 0, st>>>((__half *)x, nv, p, seed, sb);
     else
         dropout_inplace_kernel<float><<<blocks_for(nv, kEThreads), kEThreads, 0, st>>>((float *)x, nv, p, seed, sb);
     return check_launch(who);

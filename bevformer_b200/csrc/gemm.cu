@@ -29,6 +29,7 @@
 
 #include <cstdlib>
 #include <cstring>
+#include <type_traits>
 
 #include "common.cuh"
 
@@ -96,75 +97,91 @@ __device__ __forceinline__ uint64_t smem_desc_sw128(uint32_t addr, uint32_t lbo_
     return d;
 }
 
-// D[64 x N] (+)= A[64 x 16] . B[16 x N], bf16 in, fp32 accumulate in registers; kTA / kTB: operand MN-major.
+// D[64 x N] (+)= A[64 x 16] . B[16 x N], TE (bf16 | fp16) in, fp32 accumulate in registers; kTA / kTB: operand MN-major.
 // Accumulator layout (per warp w of the warpgroup, lane l): d[4j + 2h + e] = D[16 w + 8 h + l / 4][8 j + 2 (l % 4) + e].
-template <int N, int kTA, int kTB> struct Wgmma;
-template <int kTA, int kTB> struct Wgmma<64, kTA, kTB> {
+template <int N, int kTA, int kTB, typename TE> struct Wgmma;
+#define BEVF_WGMMA_N64(TY) asm volatile("{\n.reg .pred p;\nsetp.ne.b32 p, %34, 0;\n" \
+                     "wgmma.mma_async.sync.aligned.m64n64k16.f32." TY "." TY " {" \
+                     "%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, " \
+                     "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31" \
+                     "}, %32, %33, p, 1, 1, %35, %36;\n}\n" \
+                     : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), \
+                     "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), \
+                     "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), \
+                     "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]) \
+                     : "l"(da), "l"(db), "r"((int)accumulate), "n"(kTA), "n"(kTB))
+template <int kTA, int kTB, typename TE> struct Wgmma<64, kTA, kTB, TE> {
     __device__ static __forceinline__ void run(float (&d)[32], uint64_t da, uint64_t db, bool accumulate) {
-        asm volatile("{\n.reg .pred p;\nsetp.ne.b32 p, %34, 0;\n"
-                     "wgmma.mma_async.sync.aligned.m64n64k16.f32.bf16.bf16 {"
-                     "%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-                     "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31"
-                     "}, %32, %33, p, 1, 1, %35, %36;\n}\n"
-                     : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
-                     "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]),
-                     "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]),
-                     "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
-                     : "l"(da), "l"(db), "r"((int)accumulate), "n"(kTA), "n"(kTB));
+        if constexpr (std::is_same<TE, __half>::value) BEVF_WGMMA_N64("f16");
+        else BEVF_WGMMA_N64("bf16");
     }
 };
-template <int kTA, int kTB> struct Wgmma<128, kTA, kTB> {
+#undef BEVF_WGMMA_N64
+#define BEVF_WGMMA_N128(TY) asm volatile("{\n.reg .pred p;\nsetp.ne.b32 p, %66, 0;\n" \
+                     "wgmma.mma_async.sync.aligned.m64n128k16.f32." TY "." TY " {" \
+                     "%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, " \
+                     "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, " \
+                     "%32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, " \
+                     "%48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63" \
+                     "}, %64, %65, p, 1, 1, %67, %68;\n}\n" \
+                     : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), \
+                     "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), \
+                     "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), \
+                     "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), \
+                     "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), \
+                     "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), \
+                     "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), \
+                     "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63]) \
+                     : "l"(da), "l"(db), "r"((int)accumulate), "n"(kTA), "n"(kTB))
+template <int kTA, int kTB, typename TE> struct Wgmma<128, kTA, kTB, TE> {
     __device__ static __forceinline__ void run(float (&d)[64], uint64_t da, uint64_t db, bool accumulate) {
-        asm volatile("{\n.reg .pred p;\nsetp.ne.b32 p, %66, 0;\n"
-                     "wgmma.mma_async.sync.aligned.m64n128k16.f32.bf16.bf16 {"
-                     "%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-                     "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, "
-                     "%32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, "
-                     "%48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63"
-                     "}, %64, %65, p, 1, 1, %67, %68;\n}\n"
-                     : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
-                     "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]),
-                     "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]),
-                     "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]),
-                     "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]),
-                     "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]),
-                     "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]),
-                     "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
-                     : "l"(da), "l"(db), "r"((int)accumulate), "n"(kTA), "n"(kTB));
+        if constexpr (std::is_same<TE, __half>::value) BEVF_WGMMA_N128("f16");
+        else BEVF_WGMMA_N128("bf16");
     }
 };
-template <int kTA, int kTB> struct Wgmma<256, kTA, kTB> {
+#undef BEVF_WGMMA_N128
+#define BEVF_WGMMA_N256(TY) asm volatile("{\n.reg .pred p;\nsetp.ne.b32 p, %130, 0;\n" \
+                     "wgmma.mma_async.sync.aligned.m64n256k16.f32." TY "." TY " {" \
+                     "%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, " \
+                     "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, " \
+                     "%32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, " \
+                     "%48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63, " \
+                     "%64, %65, %66, %67, %68, %69, %70, %71, %72, %73, %74, %75, %76, %77, %78, %79, " \
+                     "%80, %81, %82, %83, %84, %85, %86, %87, %88, %89, %90, %91, %92, %93, %94, %95, " \
+                     "%96, %97, %98, %99, %100, %101, %102, %103, %104, %105, %106, %107, %108, %109, %110, %111, " \
+                     "%112, %113, %114, %115, %116, %117, %118, %119, %120, %121, %122, %123, %124, %125, %126, %127" \
+                     "}, %128, %129, p, 1, 1, %131, %132;\n}\n" \
+                     : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), \
+                     "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), \
+                     "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), \
+                     "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), \
+                     "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), \
+                     "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), \
+                     "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), \
+                     "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63]), \
+                     "+f"(d[64]), "+f"(d[65]), "+f"(d[66]), "+f"(d[67]), "+f"(d[68]), "+f"(d[69]), "+f"(d[70]), "+f"(d[71]), \
+                     "+f"(d[72]), "+f"(d[73]), "+f"(d[74]), "+f"(d[75]), "+f"(d[76]), "+f"(d[77]), "+f"(d[78]), "+f"(d[79]), \
+                     "+f"(d[80]), "+f"(d[81]), "+f"(d[82]), "+f"(d[83]), "+f"(d[84]), "+f"(d[85]), "+f"(d[86]), "+f"(d[87]), \
+                     "+f"(d[88]), "+f"(d[89]), "+f"(d[90]), "+f"(d[91]), "+f"(d[92]), "+f"(d[93]), "+f"(d[94]), "+f"(d[95]), \
+                     "+f"(d[96]), "+f"(d[97]), "+f"(d[98]), "+f"(d[99]), "+f"(d[100]), "+f"(d[101]), "+f"(d[102]), "+f"(d[103]), \
+                     "+f"(d[104]), "+f"(d[105]), "+f"(d[106]), "+f"(d[107]), "+f"(d[108]), "+f"(d[109]), "+f"(d[110]), "+f"(d[111]), \
+                     "+f"(d[112]), "+f"(d[113]), "+f"(d[114]), "+f"(d[115]), "+f"(d[116]), "+f"(d[117]), "+f"(d[118]), "+f"(d[119]), \
+                     "+f"(d[120]), "+f"(d[121]), "+f"(d[122]), "+f"(d[123]), "+f"(d[124]), "+f"(d[125]), "+f"(d[126]), "+f"(d[127]) \
+                     : "l"(da), "l"(db), "r"((int)accumulate), "n"(kTA), "n"(kTB))
+template <int kTA, int kTB, typename TE> struct Wgmma<256, kTA, kTB, TE> {
     __device__ static __forceinline__ void run(float (&d)[128], uint64_t da, uint64_t db, bool accumulate) {
-        asm volatile("{\n.reg .pred p;\nsetp.ne.b32 p, %130, 0;\n"
-                     "wgmma.mma_async.sync.aligned.m64n256k16.f32.bf16.bf16 {"
-                     "%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-                     "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, "
-                     "%32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, "
-                     "%48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63, "
-                     "%64, %65, %66, %67, %68, %69, %70, %71, %72, %73, %74, %75, %76, %77, %78, %79, "
-                     "%80, %81, %82, %83, %84, %85, %86, %87, %88, %89, %90, %91, %92, %93, %94, %95, "
-                     "%96, %97, %98, %99, %100, %101, %102, %103, %104, %105, %106, %107, %108, %109, %110, %111, "
-                     "%112, %113, %114, %115, %116, %117, %118, %119, %120, %121, %122, %123, %124, %125, %126, %127"
-                     "}, %128, %129, p, 1, 1, %131, %132;\n}\n"
-                     : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
-                     "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]),
-                     "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]),
-                     "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]),
-                     "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]),
-                     "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]),
-                     "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]),
-                     "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63]),
-                     "+f"(d[64]), "+f"(d[65]), "+f"(d[66]), "+f"(d[67]), "+f"(d[68]), "+f"(d[69]), "+f"(d[70]), "+f"(d[71]),
-                     "+f"(d[72]), "+f"(d[73]), "+f"(d[74]), "+f"(d[75]), "+f"(d[76]), "+f"(d[77]), "+f"(d[78]), "+f"(d[79]),
-                     "+f"(d[80]), "+f"(d[81]), "+f"(d[82]), "+f"(d[83]), "+f"(d[84]), "+f"(d[85]), "+f"(d[86]), "+f"(d[87]),
-                     "+f"(d[88]), "+f"(d[89]), "+f"(d[90]), "+f"(d[91]), "+f"(d[92]), "+f"(d[93]), "+f"(d[94]), "+f"(d[95]),
-                     "+f"(d[96]), "+f"(d[97]), "+f"(d[98]), "+f"(d[99]), "+f"(d[100]), "+f"(d[101]), "+f"(d[102]), "+f"(d[103]),
-                     "+f"(d[104]), "+f"(d[105]), "+f"(d[106]), "+f"(d[107]), "+f"(d[108]), "+f"(d[109]), "+f"(d[110]), "+f"(d[111]),
-                     "+f"(d[112]), "+f"(d[113]), "+f"(d[114]), "+f"(d[115]), "+f"(d[116]), "+f"(d[117]), "+f"(d[118]), "+f"(d[119]),
-                     "+f"(d[120]), "+f"(d[121]), "+f"(d[122]), "+f"(d[123]), "+f"(d[124]), "+f"(d[125]), "+f"(d[126]), "+f"(d[127])
-                     : "l"(da), "l"(db), "r"((int)accumulate), "n"(kTA), "n"(kTB));
+        if constexpr (std::is_same<TE, __half>::value) BEVF_WGMMA_N256("f16");
+        else BEVF_WGMMA_N256("bf16");
     }
 };
+#undef BEVF_WGMMA_N256
+
+// bias[col] as fp32 from an f32 / bf16 / fp16 vector (dt: BEVF_DTYPE_*)
+__device__ __forceinline__ float load_bias(const void *bias, int dt, int col) {
+    if (dt == BEVF_DTYPE_BF16) return __bfloat162float(reinterpret_cast<const bf16 *>(bias)[col]);
+    if (dt == BEVF_DTYPE_F16) return __half2float(reinterpret_cast<const __half *>(bias)[col]);
+    return reinterpret_cast<const float *>(bias)[col];
+}
 
 struct GemmParams {
     int M, N;              // product rows / columns
@@ -173,9 +190,9 @@ struct GemmParams {
     int splits;
     int stages;            // shared-memory ring depth
     int relu;
-    const void *bias;      // (N) f32 or bf16, or null
-    int bias_bf16;
-    const bf16 *addend;    // (M, N) bf16 added after the activation, or null
+    const void *bias;      // (N) f32 or the operand type, or null
+    int bias_dt;           // BEVF_DTYPE_* of bias
+    const void *addend;    // (M, N) in the operand type, added after the activation, or null
     void *y;               // output, row stride ldy
     int64_t ldy;
     int64_t split_stride;  // elements between the output slabs of successive splits (two-pass weight gradient)
@@ -186,7 +203,7 @@ struct GemmParams {
     int n_pad;
 };
 
-template <int BN, bool kAmn, bool kBmn>
+template <int BN, bool kAmn, bool kBmn, typename TE>
 __global__ void __launch_bounds__(kGemmThreads, 1)
 gemm_bf16_wgmma(const __grid_constant__ CUtensorMap map_a, const __grid_constant__ CUtensorMap map_b,
                 const GemmParams p) {
@@ -276,7 +293,7 @@ gemm_bf16_wgmma(const __grid_constant__ CUtensorMap map_a, const __grid_constant
                                 const uint4 v = *reinterpret_cast<const uint4 *>(sa + c * kChunk + r * 128 + ((j ^ (r & 7)) << 4));
                                 const uint32_t w4[4] = {v.x, v.y, v.z, v.w};
 #pragma unroll
-                                for (int e = 0; e < 4; ++e) { acc[c][2 * e] += bf16_lo(w4[e]); acc[c][2 * e + 1] += bf16_hi(w4[e]); }
+                                for (int e = 0; e < 4; ++e) { acc[c][2 * e] += St16<TE>::lo(w4[e]); acc[c][2 * e + 1] += St16<TE>::hi(w4[e]); }
                             }
                         }
                     }
@@ -334,7 +351,7 @@ gemm_bf16_wgmma(const __grid_constant__ CUtensorMap map_a, const __grid_constant
             wgmma_fence();
 #pragma unroll
             for (int k = 0; k < kBK / 16; ++k)
-                Wgmma<BN, kAmn, kBmn>::run(acc, da + da_step * k, db + db_step * k, (kb | k) != 0);
+                Wgmma<BN, kAmn, kBmn, TE>::run(acc, da + da_step * k, db + db_step * k, (kb | k) != 0);
             wgmma_commit();
             wgmma_wait0();
             fence_regs(acc);
@@ -350,15 +367,7 @@ gemm_bf16_wgmma(const __grid_constant__ CUtensorMap map_a, const __grid_constant
             const int col = col0 + 8 * j;
             if (col >= p.N) continue;
             float b0 = 0.f, b1 = 0.f;
-            if (p.bias) {
-                if (p.bias_bf16) {
-                    const bf16 *bp = reinterpret_cast<const bf16 *>(p.bias) + col;
-                    b0 = __bfloat162float(bp[0]); b1 = __bfloat162float(bp[1]);
-                } else {
-                    const float2 bv = __ldg(reinterpret_cast<const float2 *>(reinterpret_cast<const float *>(p.bias) + col));
-                    b0 = bv.x; b1 = bv.y;
-                }
-            }
+            if (p.bias) { b0 = load_bias(p.bias, p.bias_dt, col); b1 = load_bias(p.bias, p.bias_dt, col + 1); }
 #pragma unroll
             for (int h = 0; h < 2; ++h) {
                 const int row = row_a + 8 * h;
@@ -366,8 +375,9 @@ gemm_bf16_wgmma(const __grid_constant__ CUtensorMap map_a, const __grid_constant
                 float v0 = acc[4 * j + 2 * h] + b0, v1 = acc[4 * j + 2 * h + 1] + b1;
                 if (p.relu) { v0 = fmaxf(v0, 0.f); v1 = fmaxf(v1, 0.f); }
                 if (p.addend) {
-                    const uint32_t a2 = __ldg(reinterpret_cast<const unsigned int *>(p.addend + (size_t)row * p.N + col));
-                    v0 += bf16_lo(a2); v1 += bf16_hi(a2);
+                    const uint32_t a2 = __ldg(reinterpret_cast<const unsigned int *>(
+                        reinterpret_cast<const TE *>(p.addend) + (size_t)row * p.N + col));
+                    v0 += St16<TE>::lo(a2); v1 += St16<TE>::hi(a2);
                 }
                 const size_t off = (size_t)split * p.split_stride + (size_t)row * p.ldy + col;
                 if (p.red) {
@@ -376,7 +386,7 @@ gemm_bf16_wgmma(const __grid_constant__ CUtensorMap map_a, const __grid_constant
                 } else if (p.out_f32) {
                     *reinterpret_cast<float2 *>(reinterpret_cast<float *>(p.y) + off) = make_float2(v0, v1);
                 } else {
-                    *reinterpret_cast<uint32_t *>(reinterpret_cast<bf16 *>(p.y) + off) = pack_bf16x2(v0, v1);
+                    *reinterpret_cast<uint32_t *>(reinterpret_cast<TE *>(p.y) + off) = St16<TE>::pack(v0, v1);
                 }
             }
         }
@@ -415,9 +425,9 @@ struct WsParams {
     int stages;            // A ring depth per consumer warpgroup
     int stg_bytes;         // staging buffer per consumer warpgroup
     int relu;
-    const void *bias;      // (N) f32 or bf16, or null
-    int bias_bf16;
-    int addend;            // 1: (M, N) bf16 addend (map_add) added after the activation
+    const void *bias;      // (N) f32 or the operand type, or null
+    int bias_dt;           // BEVF_DTYPE_* of bias
+    int addend;            // 1: (M, N) addend in the operand type (map_add) added after the activation
     int out_f32;
 };
 
@@ -426,7 +436,7 @@ __device__ __forceinline__ void tma_store_2d(const CUtensorMap *map, const void 
                  ::"l"(map), "r"(smem_u32(src)), "r"(c0), "r"(c1) : "memory");
 }
 
-template <int BN, bool kBmn>
+template <int BN, bool kBmn, typename TE>
 __global__ void __launch_bounds__(kGemmThreads, 1)
 gemm_ws_wgmma(const __grid_constant__ CUtensorMap map_a, const __grid_constant__ CUtensorMap map_w,
               const __grid_constant__ CUtensorMap map_y, const __grid_constant__ CUtensorMap map_add,
@@ -520,9 +530,7 @@ gemm_ws_wgmma(const __grid_constant__ CUtensorMap map_a, const __grid_constant__
     for (int i = threadIdx.x - 128; i < BN; i += 256) {
         const int col = col0 + i;
         float b = 0.f;
-        if (p.bias && col < p.N)
-            b = p.bias_bf16 ? __bfloat162float(reinterpret_cast<const bf16 *>(p.bias)[col])
-                            : reinterpret_cast<const float *>(p.bias)[col];
+        if (p.bias && col < p.N) b = load_bias(p.bias, p.bias_dt, col);
         sbias[i] = b;
     }
     asm volatile("bar.sync 3, 256;" ::: "memory");
@@ -537,7 +545,7 @@ gemm_ws_wgmma(const __grid_constant__ CUtensorMap map_a, const __grid_constant__
             wgmma_fence();
 #pragma unroll
             for (int k = 0; k < kBK / 16; ++k)
-                Wgmma<BN, 0, kBmn>::run(acc, da + 2 * k, db + db_step * k, (kb | k) != 0);
+                Wgmma<BN, 0, kBmn, TE>::run(acc, da + 2 * k, db + db_step * k, (kb | k) != 0);
             wgmma_commit();
             if (prev >= 0) {
                 // the group of k-block kb - 1 has retired: its A stage can be refilled
@@ -565,11 +573,11 @@ gemm_ws_wgmma(const __grid_constant__ CUtensorMap map_a, const __grid_constant__
                 float v0 = acc[4 * j + 2 * h] + b0, v1 = acc[4 * j + 2 * h + 1] + b1;
                 if (p.relu) { v0 = fmaxf(v0, 0.f); v1 = fmaxf(v1, 0.f); }
                 if (p.addend) {
-                    // bf16 box j / 8, 16 B unit j % 8 of row r, stored at unit (j % 8) ^ (r % 8)
+                    // 16-bit box j / 8, 16 B unit j % 8 of row r, stored at unit (j % 8) ^ (r % 8)
                     const int r = r0 + 8 * h;
                     const uint32_t a2 = *reinterpret_cast<const uint32_t *>(
                         stg + (j >> 3) * kWsBoxBytes + r * 128 + (((j & 7) ^ (r & 7)) << 4) + 2 * cq);
-                    v0 += bf16_lo(a2); v1 += bf16_hi(a2);
+                    v0 += St16<TE>::lo(a2); v1 += St16<TE>::hi(a2);
                 }
                 acc[4 * j + 2 * h] = v0; acc[4 * j + 2 * h + 1] = v1;
             }
@@ -594,7 +602,7 @@ gemm_ws_wgmma(const __grid_constant__ CUtensorMap map_a, const __grid_constant__
                                                     4 * (cq & 3)) = make_float2(v0, v1);
                     } else {
                         *reinterpret_cast<uint32_t *>(stg + (j >> 3) * kWsBoxBytes + r * 128 +
-                                                      (((j & 7) ^ (r & 7)) << 4) + 2 * cq) = pack_bf16x2(v0, v1);
+                                                      (((j & 7) ^ (r & 7)) << 4) + 2 * cq) = St16<TE>::pack(v0, v1);
                     }
                 }
             }
@@ -635,7 +643,7 @@ wgrad_reduce_kernel(const float *__restrict__ ws, const float *__restrict__ ws_b
             a.x += v.x; a.y += v.y; a.z += v.z; a.w += v.w;
         }
         if constexpr (sizeof(TO) == 2) {
-            *reinterpret_cast<uint2 *>(dw + (size_t)n * K + c) = make_uint2(pack_bf16x2(a.x, a.y), pack_bf16x2(a.z, a.w));
+            *reinterpret_cast<uint2 *>(dw + (size_t)n * K + c) = make_uint2(St16<TO>::pack(a.x, a.y), St16<TO>::pack(a.z, a.w));
         } else if constexpr (kAcc) {
             float4 *d = reinterpret_cast<float4 *>(dw + (size_t)n * K + c);
             const float4 o = *d;
@@ -647,7 +655,7 @@ wgrad_reduce_kernel(const float *__restrict__ ws, const float *__restrict__ ws_b
         const int n = (int)(t - total);
         float a = 0.f;
         for (int s2 = 0; s2 < splits; ++s2) a += ws_b[(size_t)s2 * n_pad + n];
-        if constexpr (sizeof(TO) == 2) db[n] = __float2bfloat16_rn(a);
+        if constexpr (sizeof(TO) == 2) db[n] = St16<TO>::from_f(a);
         else if constexpr (kAcc) db[n] += a;
         else db[n] = a;
     }
@@ -672,18 +680,20 @@ static EncodeTiledFn encode_tiled_fn() {
     return fn;
 }
 
-// row-major (rows, cols) bf16 (or fp32); box = box_rows x 128 B, SWIZZLE_128B; out-of-range rows and columns of a
-// box read as zeros (and still count towards the transaction bytes), and are not written by a store
-static int make_map_2d(CUtensorMap *map, const void *ptr, uint64_t rows, uint64_t cols, uint32_t box_rows,
-                       bool f32 = false) {
+// row-major (rows, cols) of BEVF_DTYPE_* dt; box = box_rows x 128 B, SWIZZLE_128B; out-of-range rows and columns of
+// a box read as zeros (and still count towards the transaction bytes), and are not written by a store
+static int make_map_2d(CUtensorMap *map, const void *ptr, uint64_t rows, uint64_t cols, uint32_t box_rows, int dt) {
     EncodeTiledFn encode = encode_tiled_fn();
     if (!encode) return -1;
+    const bool f32 = dt == BEVF_DTYPE_F32;
     const uint32_t esz = f32 ? 4 : 2;
     cuuint64_t dims[2] = {cols, rows};
     cuuint64_t strides[1] = {cols * esz};
     cuuint32_t box[2] = {128 / esz, box_rows};
     cuuint32_t estr[2] = {1, 1};
-    CUresult r = encode(map, f32 ? CU_TENSOR_MAP_DATA_TYPE_FLOAT32 : CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2,
+    const CUtensorMapDataType ty = f32 ? CU_TENSOR_MAP_DATA_TYPE_FLOAT32
+                                 : dt == BEVF_DTYPE_F16 ? CU_TENSOR_MAP_DATA_TYPE_FLOAT16 : CU_TENSOR_MAP_DATA_TYPE_BFLOAT16;
+    CUresult r = encode(map, ty, 2,
                         const_cast<void *>(ptr), dims,
                         strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
                         CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
@@ -693,7 +703,7 @@ static int make_map_2d(CUtensorMap *map, const void *ptr, uint64_t rows, uint64_
 
 // Launch of one instantiation; the operand maps are built by the caller.  A is 128 x 64 per k-block (K-major:
 // one 128-row box; MN-major: two 64 x 64 boxes), B is BN x 64 (K-major: one BN-row box; MN-major: BN / 64 boxes).
-template <int BN, bool kAmn, bool kBmn>
+template <int BN, bool kAmn, bool kBmn, typename TE>
 static int launch_gemm(const char *who, const CUtensorMap &map_a, const CUtensorMap &map_b, GemmParams p,
                        cudaStream_t st) {
     constexpr int kStageBytes = kBM * 128 + BN * 128;
@@ -703,7 +713,7 @@ static int launch_gemm(const char *who, const CUtensorMap &map_a, const CUtensor
     const size_t smem = 1024 + (size_t)stages * kStageBytes + 2 * kMaxStages * 8;
     static bool configured = false;
     if (!configured) {
-        if (cudaFuncSetAttribute(gemm_bf16_wgmma<BN, kAmn, kBmn>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+        if (cudaFuncSetAttribute(gemm_bf16_wgmma<BN, kAmn, kBmn, TE>, cudaFuncAttributeMaxDynamicSharedMemorySize,
                                  (int)smem) != cudaSuccess) {
             cudaGetLastError();
             return fail("%s: cannot reserve shared memory for the GEMM", who);
@@ -712,7 +722,7 @@ static int launch_gemm(const char *who, const CUtensorMap &map_a, const CUtensor
     }
     const int units = ((p.M + kBM - 1) / kBM) * ((p.N + BN - 1) / BN) * p.splits;
     const int grid = units < device_sms() ? units : device_sms();
-    gemm_bf16_wgmma<BN, kAmn, kBmn><<<grid, kGemmThreads, smem, st>>>(map_a, map_b, p);
+    gemm_bf16_wgmma<BN, kAmn, kBmn, TE><<<grid, kGemmThreads, smem, st>>>(map_a, map_b, p);
     return check_launch(who);
 }
 
@@ -725,7 +735,7 @@ static int ws_block(int N, int R) {
     return bn * R * 2 <= kWsWeightMax ? bn : 0;
 }
 
-template <int BN, bool kBmn>
+template <int BN, bool kBmn, typename TE>
 static int launch_ws(const char *who, const CUtensorMap &map_a, const CUtensorMap &map_w, const CUtensorMap &map_y,
                      const CUtensorMap &map_add, WsParams p, cudaStream_t st) {
     constexpr int kSmemMax = 227 * 1024;
@@ -740,7 +750,7 @@ static int launch_ws(const char *who, const CUtensorMap &map_a, const CUtensorMa
     const size_t smem = 1024 + (size_t)w_bytes + 2 * p.stg_bytes + 2 * (size_t)stages * kWsBoxBytes + kBarBytes;
     static bool configured = false;
     if (!configured) {
-        if (cudaFuncSetAttribute(gemm_ws_wgmma<BN, kBmn>, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmemMax) !=
+        if (cudaFuncSetAttribute(gemm_ws_wgmma<BN, kBmn, TE>, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmemMax) !=
             cudaSuccess) {
             cudaGetLastError();
             return fail("%s: cannot reserve shared memory for the GEMM", who);
@@ -752,38 +762,42 @@ static int launch_ws(const char *who, const CUtensorMap &map_a, const CUtensorMa
     p.groups = device_sms() / p.tiles_n;
     if (p.groups > p.tiles_m) p.groups = p.tiles_m;
     if (p.groups < 1) p.groups = 1;
-    gemm_ws_wgmma<BN, kBmn><<<p.groups * p.tiles_n, kGemmThreads, smem, st>>>(map_a, map_w, map_y, map_add, p);
+    gemm_ws_wgmma<BN, kBmn, TE><<<p.groups * p.tiles_n, kGemmThreads, smem, st>>>(map_a, map_w, map_y, map_add, p);
     return check_launch(who);
 }
 
 // Y (M, N) = act(A (M, R) . B + bias) (+ addend) on the weight-stationary kernel; B is W (N, R) for the forward
 // product, or W (R, N) read in place (MN-major) for the input gradient.
-static int linear_ws(const char *who, int bn, bool b_mn, const void *a, const void *w, const void *bias, int bias_bf16,
+template <typename TE> constexpr int dtype_of() { return std::is_same<TE, __half>::value ? BEVF_DTYPE_F16 : BEVF_DTYPE_BF16; }
+
+template <typename TE>
+static int linear_ws(const char *who, int bn, bool b_mn, const void *a, const void *w, const void *bias, int bias_dt,
                      const void *addend, void *y, bool out_f32, int M, int N, int R, int relu, cudaStream_t st) {
+    constexpr int dt = dtype_of<TE>();
     CUtensorMap map_a, map_w, map_y, map_add;
-    if (int e = make_map_2d(&map_a, a, (uint64_t)M, (uint64_t)R, kWsRows))
+    if (int e = make_map_2d(&map_a, a, (uint64_t)M, (uint64_t)R, kWsRows, dt))
         return fail("%s: cuTensorMapEncodeTiled(A) failed (%lld)", who, e);
-    if (int e = b_mn ? make_map_2d(&map_w, w, (uint64_t)R, (uint64_t)N, 64)
-                     : make_map_2d(&map_w, w, (uint64_t)N, (uint64_t)R, (uint32_t)bn))
+    if (int e = b_mn ? make_map_2d(&map_w, w, (uint64_t)R, (uint64_t)N, 64, dt)
+                     : make_map_2d(&map_w, w, (uint64_t)N, (uint64_t)R, (uint32_t)bn, dt))
         return fail("%s: cuTensorMapEncodeTiled(B) failed (%lld)", who, e);
-    if (int e = make_map_2d(&map_y, y, (uint64_t)M, (uint64_t)N, kWsRows, out_f32))
+    if (int e = make_map_2d(&map_y, y, (uint64_t)M, (uint64_t)N, kWsRows, out_f32 ? BEVF_DTYPE_F32 : dt))
         return fail("%s: cuTensorMapEncodeTiled(Y) failed (%lld)", who, e);
     map_add = map_y;
     if (addend)
-        if (int e = make_map_2d(&map_add, addend, (uint64_t)M, (uint64_t)N, kWsRows))
+        if (int e = make_map_2d(&map_add, addend, (uint64_t)M, (uint64_t)N, kWsRows, dt))
             return fail("%s: cuTensorMapEncodeTiled(addend) failed (%lld)", who, e);
     WsParams p;
     memset(&p, 0, sizeof(p));
     p.M = M; p.N = N; p.R = R;
-    p.relu = relu; p.bias = bias; p.bias_bf16 = bias_bf16;
+    p.relu = relu; p.bias = bias; p.bias_dt = bias_dt;
     p.addend = addend != nullptr; p.out_f32 = out_f32;
     switch (bn * 2 + (int)b_mn) {
-        case 512: return launch_ws<256, false>(who, map_a, map_w, map_y, map_add, p, st);
-        case 513: return launch_ws<256, true>(who, map_a, map_w, map_y, map_add, p, st);
-        case 256: return launch_ws<128, false>(who, map_a, map_w, map_y, map_add, p, st);
-        case 257: return launch_ws<128, true>(who, map_a, map_w, map_y, map_add, p, st);
-        case 128: return launch_ws<64, false>(who, map_a, map_w, map_y, map_add, p, st);
-        case 129: return launch_ws<64, true>(who, map_a, map_w, map_y, map_add, p, st);
+        case 512: return launch_ws<256, false, TE>(who, map_a, map_w, map_y, map_add, p, st);
+        case 513: return launch_ws<256, true, TE>(who, map_a, map_w, map_y, map_add, p, st);
+        case 256: return launch_ws<128, false, TE>(who, map_a, map_w, map_y, map_add, p, st);
+        case 257: return launch_ws<128, true, TE>(who, map_a, map_w, map_y, map_add, p, st);
+        case 128: return launch_ws<64, false, TE>(who, map_a, map_w, map_y, map_add, p, st);
+        case 129: return launch_ws<64, true, TE>(who, map_a, map_w, map_y, map_add, p, st);
     }
     return fail("%s: no weight-stationary tile for this shape", who);
 }
@@ -800,21 +814,13 @@ static GemmParams base_params(int M, int N, int R) {
 
 using namespace bevf;
 
-static int linear_dgrad_impl(const char *who, const void *dy, const void *w, const void *addend, void *dx, int64_t M,
-                             int N, int K, void *stream);
+// operand type of the *_dt entry points: bf16 or fp16
+static bool operand_dtype_ok(int dtype) { return dtype == BEVF_DTYPE_BF16 || dtype == BEVF_DTYPE_F16; }
 
-extern "C" int bevf_linear_dgrad(const void *dy, const void *w, void *dx, int64_t M, int N, int K, void *stream) {
-    return linear_dgrad_impl("bevf_linear_dgrad", dy, w, nullptr, dx, M, N, K, stream);
-}
-
-extern "C" int bevf_linear_dgrad_acc(const void *dy, const void *w, const void *addend, void *dx, int64_t M, int N,
-                                     int K, void *stream) {
-    if (addend && !aligned16(addend)) return fail("%s: addend must be 16-byte aligned", "bevf_linear_dgrad_acc");
-    return linear_dgrad_impl("bevf_linear_dgrad_acc", dy, w, addend, dx, M, N, K, stream);
-}
-
+template <typename TE>
 static int linear_dgrad_impl(const char *who, const void *dy, const void *w, const void *addend, void *dx, int64_t M,
                              int N, int K, void *stream) {
+    constexpr int dt = dtype_of<TE>();
     if (M < 0 || N <= 0 || K <= 0) return fail("%s: bad dimension", who);
     if (M == 0) return 0;
     if (!dy || !w || !dx) return fail("%s: null pointer argument", who);
@@ -824,23 +830,51 @@ static int linear_dgrad_impl(const char *who, const void *dy, const void *w, con
     // dX (M, K) = dY (M, N) . W (N, K): A = dY K-major, B = W with its output columns contiguous (MN-major)
     cudaStream_t st = (cudaStream_t)stream;
     if (int bn = ws_block(K, N))
-        return linear_ws(who, bn, true, dy, w, nullptr, 0, addend, dx, false, (int)M, K, N, 0, st);
+        return linear_ws<TE>(who, bn, true, dy, w, nullptr, BEVF_DTYPE_F32, addend, dx, false, (int)M, K, N, 0, st);
     CUtensorMap map_a, map_b;
-    if (int e = make_map_2d(&map_a, dy, (uint64_t)M, (uint64_t)N, kBM))
+    if (int e = make_map_2d(&map_a, dy, (uint64_t)M, (uint64_t)N, kBM, dt))
         return fail("%s: cuTensorMapEncodeTiled(A) failed (%lld)", who, e);
-    if (int e = make_map_2d(&map_b, w, (uint64_t)N, (uint64_t)K, 64))
+    if (int e = make_map_2d(&map_b, w, (uint64_t)N, (uint64_t)K, 64, dt))
         return fail("%s: cuTensorMapEncodeTiled(B) failed (%lld)", who, e);
     GemmParams p = base_params((int)M, K, N);
-    p.addend = reinterpret_cast<const bf16 *>(addend);
+    p.addend = addend;
     p.y = dx;
-    return K % 128 == 0 ? launch_gemm<128, false, true>(who, map_a, map_b, p, st)
-                        : launch_gemm<64, false, true>(who, map_a, map_b, p, st);
+    return K % 128 == 0 ? launch_gemm<128, false, true, TE>(who, map_a, map_b, p, st)
+                        : launch_gemm<64, false, true, TE>(who, map_a, map_b, p, st);
 }
 
-extern "C" int bevf_linear_forward(const void *x, const void *w, const void *bias, int bias_dtype,
-                                   const void *residual, void *y, int y_dtype, int64_t M, int N, int K,
-                                   int relu, void *stream) {
-    const char *who = "bevf_linear_forward";
+static int linear_dgrad_dispatch(const char *who, const void *dy, const void *w, const void *addend, void *dx,
+                                 int64_t M, int N, int K, int dtype, void *stream) {
+    if (addend && !aligned16(addend)) return fail("%s: addend must be 16-byte aligned", who);
+    if (dtype == BEVF_DTYPE_F16) return linear_dgrad_impl<__half>(who, dy, w, addend, dx, M, N, K, stream);
+    if (dtype == BEVF_DTYPE_BF16) return linear_dgrad_impl<bf16>(who, dy, w, addend, dx, M, N, K, stream);
+    return fail("%s: unsupported operand dtype code (bf16 or fp16)", who);
+}
+
+extern "C" int bevf_linear_dgrad(const void *dy, const void *w, void *dx, int64_t M, int N, int K, void *stream) {
+    return linear_dgrad_dispatch("bevf_linear_dgrad", dy, w, nullptr, dx, M, N, K, BEVF_DTYPE_BF16, stream);
+}
+
+extern "C" int bevf_linear_dgrad_dt(const void *dy, const void *w, void *dx, int64_t M, int N, int K, int dtype,
+                                    void *stream) {
+    return linear_dgrad_dispatch("bevf_linear_dgrad_dt", dy, w, nullptr, dx, M, N, K, dtype, stream);
+}
+
+extern "C" int bevf_linear_dgrad_acc(const void *dy, const void *w, const void *addend, void *dx, int64_t M, int N,
+                                     int K, void *stream) {
+    return linear_dgrad_dispatch("bevf_linear_dgrad_acc", dy, w, addend, dx, M, N, K, BEVF_DTYPE_BF16, stream);
+}
+
+extern "C" int bevf_linear_dgrad_acc_dt(const void *dy, const void *w, const void *addend, void *dx, int64_t M, int N,
+                                        int K, int dtype, void *stream) {
+    return linear_dgrad_dispatch("bevf_linear_dgrad_acc_dt", dy, w, addend, dx, M, N, K, dtype, stream);
+}
+
+template <typename TE>
+static int linear_forward_impl(const char *who, const void *x, const void *w, const void *bias, int bias_dtype,
+                               const void *residual, void *y, int y_dtype, int64_t M, int N, int K, int relu,
+                               void *stream) {
+    constexpr int dt = dtype_of<TE>();
     if (M < 0 || N <= 0 || K <= 0) return fail("%s: bad dimension", who);
     if (M == 0) return 0;
     if (!x || !w || !y) return fail("%s: null pointer argument", who);
@@ -850,26 +884,44 @@ extern "C" int bevf_linear_forward(const void *x, const void *w, const void *bia
     if (!aligned16(x) || !aligned16(w) || !aligned16(y) || (bias && !aligned16(bias)) ||
         (residual && !aligned16(residual)))
         return fail("%s: pointers must be 16-byte aligned", who);
-    if (y_dtype != BEVF_DTYPE_BF16 && y_dtype != BEVF_DTYPE_F32) return fail("%s: unsupported dtype code", who);
-    if (bias && bias_dtype != BEVF_DTYPE_BF16 && bias_dtype != BEVF_DTYPE_F32)
+    if (y_dtype != dt && y_dtype != BEVF_DTYPE_F32) return fail("%s: unsupported dtype code", who);
+    if (bias && bias_dtype != dt && bias_dtype != BEVF_DTYPE_F32)
         return fail("%s: unsupported bias dtype code", who);
     cudaStream_t st = (cudaStream_t)stream;
     if (int bn = ws_block(N, K))
-        return linear_ws(who, bn, false, x, w, bias, bias_dtype == BEVF_DTYPE_BF16, residual, y,
-                         y_dtype == BEVF_DTYPE_F32, (int)M, N, K, relu, st);
+        return linear_ws<TE>(who, bn, false, x, w, bias, bias_dtype, residual, y, y_dtype == BEVF_DTYPE_F32, (int)M, N,
+                             K, relu, st);
     // a column tile of 128 unless N is small (a partial last tile is clipped in the epilogue)
     const bool wide = N > 64;
     CUtensorMap map_a, map_b;
-    if (int e = make_map_2d(&map_a, x, (uint64_t)M, (uint64_t)K, kBM))
+    if (int e = make_map_2d(&map_a, x, (uint64_t)M, (uint64_t)K, kBM, dt))
         return fail("%s: cuTensorMapEncodeTiled(A) failed (%lld)", who, e);
-    if (int e = make_map_2d(&map_b, w, (uint64_t)N, (uint64_t)K, wide ? 128 : 64))
+    if (int e = make_map_2d(&map_b, w, (uint64_t)N, (uint64_t)K, wide ? 128 : 64, dt))
         return fail("%s: cuTensorMapEncodeTiled(B) failed (%lld)", who, e);
     GemmParams p = base_params((int)M, N, K);
-    p.relu = relu; p.bias = bias; p.bias_bf16 = bias_dtype == BEVF_DTYPE_BF16;
-    p.addend = reinterpret_cast<const bf16 *>(residual);
+    p.relu = relu; p.bias = bias; p.bias_dt = bias_dtype;
+    p.addend = residual;
     p.y = y; p.out_f32 = y_dtype == BEVF_DTYPE_F32;
-    return wide ? launch_gemm<128, false, false>(who, map_a, map_b, p, st)
-                : launch_gemm<64, false, false>(who, map_a, map_b, p, st);
+    return wide ? launch_gemm<128, false, false, TE>(who, map_a, map_b, p, st)
+                : launch_gemm<64, false, false, TE>(who, map_a, map_b, p, st);
+}
+
+extern "C" int bevf_linear_forward_dt(const void *x, const void *w, const void *bias, int bias_dtype,
+                                      const void *residual, void *y, int y_dtype, int64_t M, int N, int K, int relu,
+                                      int dtype, void *stream) {
+    const char *who = "bevf_linear_forward_dt";
+    if (dtype == BEVF_DTYPE_F16)
+        return linear_forward_impl<__half>(who, x, w, bias, bias_dtype, residual, y, y_dtype, M, N, K, relu, stream);
+    if (dtype == BEVF_DTYPE_BF16)
+        return linear_forward_impl<bf16>(who, x, w, bias, bias_dtype, residual, y, y_dtype, M, N, K, relu, stream);
+    return fail("%s: unsupported operand dtype code (bf16 or fp16)", who);
+}
+
+extern "C" int bevf_linear_forward(const void *x, const void *w, const void *bias, int bias_dtype,
+                                   const void *residual, void *y, int y_dtype, int64_t M, int N, int K,
+                                   int relu, void *stream) {
+    return linear_forward_impl<bf16>("bevf_linear_forward", x, w, bias, bias_dtype, residual, y, y_dtype, M, N, K,
+                                     relu, stream);
 }
 
 // Plan of the weight gradient, shared by the workspace query and the launches: tile width along K, number of
@@ -886,19 +938,20 @@ static void wgrad_plan(int64_t M, int N, int K, int &bn, int &splits, int &rows,
 }
 
 // dW (N, K) = dY^T . X: both operands MN-major (dY (M, N) and X (M, K) read row-major, reduction over M)
+template <typename TE>
 static int launch_wgrad(const char *who, const void *dy, const void *x, GemmParams p, int bn, cudaStream_t st) {
+    constexpr int dt = dtype_of<TE>();
     CUtensorMap map_a, map_b;
-    if (int e = make_map_2d(&map_a, dy, (uint64_t)p.R, (uint64_t)p.M, 64))
+    if (int e = make_map_2d(&map_a, dy, (uint64_t)p.R, (uint64_t)p.M, 64, dt))
         return fail("%s: cuTensorMapEncodeTiled(dY) failed (%lld)", who, e);
-    if (int e = make_map_2d(&map_b, x, (uint64_t)p.R, (uint64_t)p.N, 64))
+    if (int e = make_map_2d(&map_b, x, (uint64_t)p.R, (uint64_t)p.N, 64, dt))
         return fail("%s: cuTensorMapEncodeTiled(X) failed (%lld)", who, e);
-    return bn == 128 ? launch_gemm<128, true, true>(who, map_a, map_b, p, st)
-                     : launch_gemm<64, true, true>(who, map_a, map_b, p, st);
+    return bn == 128 ? launch_gemm<128, true, true, TE>(who, map_a, map_b, p, st)
+                     : launch_gemm<64, true, true, TE>(who, map_a, map_b, p, st);
 }
 
-extern "C" int bevf_linear_wgrad(const void *dy, const void *x, float *dw, float *db, int64_t M, int N,
-                                 int K, void *stream) {
-    const char *who = "bevf_linear_wgrad";
+static int linear_wgrad_impl(const char *who, const void *dy, const void *x, float *dw, float *db, int64_t M, int N,
+                             int K, int dtype, void *stream) {
     if (M < 0 || N <= 0 || K <= 0) return fail("%s: bad dimension", who);
     if (M == 0) return 0;
     if (!dy || !x || !dw) return fail("%s: null pointer argument", who);
@@ -906,13 +959,26 @@ extern "C" int bevf_linear_wgrad(const void *dy, const void *x, float *dw, float
     if (db && !aligned16(db)) return fail("%s: pointers must be 16-byte aligned", who);
     if (M >= (1ll << 31)) return fail("%s: M too large", who);
     if (!aligned16(dy) || !aligned16(x) || !aligned16(dw)) return fail("%s: pointers must be 16-byte aligned", who);
+    if (!operand_dtype_ok(dtype)) return fail("%s: unsupported operand dtype code (bf16 or fp16)", who);
     int bn, splits, rows, n_pad;
     wgrad_plan(M, N, K, bn, splits, rows, n_pad);
     GemmParams p = base_params(N, K, (int)M);
     p.rows_per_split = rows; p.splits = splits;
     p.y = dw; p.ldy = K; p.out_f32 = 1; p.red = 1;      // every split reduces its partial tile into dW
     p.db = db;
-    return launch_wgrad(who, dy, x, p, bn, (cudaStream_t)stream);
+    cudaStream_t st = (cudaStream_t)stream;
+    return dtype == BEVF_DTYPE_F16 ? launch_wgrad<__half>(who, dy, x, p, bn, st)
+                                   : launch_wgrad<bf16>(who, dy, x, p, bn, st);
+}
+
+extern "C" int bevf_linear_wgrad(const void *dy, const void *x, float *dw, float *db, int64_t M, int N,
+                                 int K, void *stream) {
+    return linear_wgrad_impl("bevf_linear_wgrad", dy, x, dw, db, M, N, K, BEVF_DTYPE_BF16, stream);
+}
+
+extern "C" int bevf_linear_wgrad_dt(const void *dy, const void *x, float *dw, float *db, int64_t M, int N, int K,
+                                    int dtype, void *stream) {
+    return linear_wgrad_impl("bevf_linear_wgrad_dt", dy, x, dw, db, M, N, K, dtype, stream);
 }
 
 extern "C" int64_t bevf_linear_wgrad_workspace_bytes(int64_t M, int N, int K) {
@@ -925,14 +991,16 @@ extern "C" int64_t bevf_linear_wgrad_workspace_bytes(int64_t M, int N, int K) {
 // grad_dtype, or accumulate != 0: dw / db fp32 and added into
 static int wgrad_two_pass(const char *who, const void *dy, const void *x, void *dw, void *db, int grad_dtype,
                           int accumulate, void *workspace, int64_t workspace_bytes, int64_t M, int N, int K,
-                          void *stream) {
+                          int dtype, void *stream) {
     if (M <= 0 || N <= 0 || K <= 0) return fail("%s: bad dimension", who);
     if (!dy || !x || !dw || !workspace) return fail("%s: null pointer argument", who);
     if (K % 64 != 0 || N % 8 != 0) return fail("%s: K must be a multiple of 64 and N of 8", who);
     if (M >= (1ll << 31)) return fail("%s: M too large", who);
     if (!aligned16(dy) || !aligned16(x) || !aligned16(dw) || !aligned16(workspace))
         return fail("%s: pointers must be 16-byte aligned", who);
-    if (grad_dtype != BEVF_DTYPE_BF16 && grad_dtype != BEVF_DTYPE_F32) return fail("%s: unsupported dtype code", who);
+    if (!operand_dtype_ok(dtype)) return fail("%s: unsupported operand dtype code (bf16 or fp16)", who);
+    if (grad_dtype != BEVF_DTYPE_BF16 && grad_dtype != BEVF_DTYPE_F16 && grad_dtype != BEVF_DTYPE_F32)
+        return fail("%s: unsupported dtype code", who);
     if (workspace_bytes < bevf_linear_wgrad_workspace_bytes(M, N, K))
         return fail("%s: workspace too small (need %lld bytes)", who, bevf_linear_wgrad_workspace_bytes(M, N, K));
     int bn, splits, rows, n_pad;
@@ -945,7 +1013,9 @@ static int wgrad_two_pass(const char *who, const void *dy, const void *x, void *
     p.y = ws; p.ldy = K; p.split_stride = (int64_t)n_pad * K; p.out_f32 = 1;
     p.db_ws = db ? ws_b : nullptr; p.n_pad = n_pad;
     cudaStream_t cs = (cudaStream_t)stream;
-    if (int e = launch_wgrad(who, dy, x, p, bn, cs)) return e;
+    if (int e = dtype == BEVF_DTYPE_F16 ? launch_wgrad<__half>(who, dy, x, p, bn, cs)
+                                       : launch_wgrad<bf16>(who, dy, x, p, bn, cs))
+        return e;
     // pass 2: sum the slabs in the parameter's dtype
     const long long total = (long long)N * (K / 4) + (db ? N : 0);
     const unsigned rgrid = (unsigned)((total + 255) / 256);
@@ -953,6 +1023,8 @@ static int wgrad_two_pass(const char *who, const void *dy, const void *x, void *
         wgrad_reduce_kernel<float, true><<<rgrid, 256, 0, cs>>>(ws, ws_b, (float *)dw, (float *)db, N, K, n_pad, splits);
     else if (grad_dtype == BEVF_DTYPE_BF16)
         wgrad_reduce_kernel<bf16><<<rgrid, 256, 0, cs>>>(ws, ws_b, (bf16 *)dw, (bf16 *)db, N, K, n_pad, splits);
+    else if (grad_dtype == BEVF_DTYPE_F16)
+        wgrad_reduce_kernel<__half><<<rgrid, 256, 0, cs>>>(ws, ws_b, (__half *)dw, (__half *)db, N, K, n_pad, splits);
     else
         wgrad_reduce_kernel<float><<<rgrid, 256, 0, cs>>>(ws, ws_b, (float *)dw, (float *)db, N, K, n_pad, splits);
     return check_launch(who);
@@ -962,11 +1034,24 @@ extern "C" int bevf_linear_wgrad_out(const void *dy, const void *x, void *dw, vo
                                      void *workspace, int64_t workspace_bytes, int64_t M, int N, int K,
                                      void *stream) {
     return wgrad_two_pass("bevf_linear_wgrad_out", dy, x, dw, db, grad_dtype, 0, workspace, workspace_bytes, M, N, K,
-                          stream);
+                          BEVF_DTYPE_BF16, stream);
+}
+
+extern "C" int bevf_linear_wgrad_out_dt(const void *dy, const void *x, void *dw, void *db, int grad_dtype,
+                                        void *workspace, int64_t workspace_bytes, int64_t M, int N, int K, int dtype,
+                                        void *stream) {
+    return wgrad_two_pass("bevf_linear_wgrad_out_dt", dy, x, dw, db, grad_dtype, 0, workspace, workspace_bytes, M, N,
+                          K, dtype, stream);
 }
 
 extern "C" int bevf_linear_wgrad_into(const void *dy, const void *x, float *dw, float *db, void *workspace,
                                       int64_t workspace_bytes, int64_t M, int N, int K, void *stream) {
     return wgrad_two_pass("bevf_linear_wgrad_into", dy, x, dw, db, BEVF_DTYPE_F32, 1, workspace, workspace_bytes, M, N,
-                          K, stream);
+                          K, BEVF_DTYPE_BF16, stream);
+}
+
+extern "C" int bevf_linear_wgrad_into_dt(const void *dy, const void *x, float *dw, float *db, void *workspace,
+                                         int64_t workspace_bytes, int64_t M, int N, int K, int dtype, void *stream) {
+    return wgrad_two_pass("bevf_linear_wgrad_into_dt", dy, x, dw, db, BEVF_DTYPE_F32, 1, workspace, workspace_bytes,
+                          M, N, K, dtype, stream);
 }

@@ -4,7 +4,7 @@
 //   fx_bounds_launch       max|attn| and max|grad_out| over the launch's live rows as sign-cleared float bits in two
 //                          device words (an unsigned maximum: order-free, and NaN / inf dominate every finite value)
 //   bevf_msda_fx_frac_bits the fraction bits K a launch can use without any possibility of overflow
-//   bevf_msda_fx_convert   int64 accumulators -> fp32 / bf16 gradient, written or ADDED into the caller's buffer
+//   bevf_msda_fx_convert   int64 accumulators -> fp32 / bf16 / fp16 gradient, written or ADDED into the caller's buffer
 // The scale is a power of two read from device words (no host synchronisation: capturable in a CUDA graph).
 #include "common.cuh"
 
@@ -16,6 +16,7 @@ __device__ __forceinline__ unsigned abs_bits(float x) { return __float_as_uint(x
 __device__ __forceinline__ unsigned abs_bits(bf16 x) {
     return ((unsigned)__bfloat16_as_ushort(x) << 16) & 0x7fffffffu;
 }
+__device__ __forceinline__ unsigned abs_bits(__half x) { return abs_bits(__half2float(x)); }
 
 // one warp per query row; rows with row_map < 0 (unused rows of a fixed-capacity list, never written) are skipped
 template <typename TG>
@@ -51,8 +52,8 @@ fx_convert_kernel(const long long *__restrict__ fx, const unsigned *__restrict__
     for (long long i = (long long)blockIdx.x * kFxThreads + threadIdx.x; i < n; i += (long long)gridDim.x * kFxThreads) {
         float v = finite ? (float)((double)__ldg(fx + i) * inv) : __int_as_float(0x7fffffff);
         if constexpr (sizeof(TO) == 2) {
-            if constexpr (kAcc) v += __bfloat162float(out[i]);
-            out[i] = __float2bfloat16_rn(v);
+            if constexpr (kAcc) v += St16<TO>::to_f(out[i]);
+            out[i] = St16<TO>::from_f(v);
         } else {
             if constexpr (kAcc) v += out[i];
             out[i] = v;
@@ -74,6 +75,8 @@ int fx_bounds_launch(const char *who, const float *attn, const void *grad_out, i
     const unsigned grid = fx_grid(qrows, kFxThreads / 32);
     if (grad_out_dtype == BEVF_DTYPE_BF16)
         fx_bounds_kernel<bf16><<<grid, kFxThreads, 0, st>>>(attn, (const bf16 *)grad_out, row_map, qrows, na, ng, bounds);
+    else if (grad_out_dtype == BEVF_DTYPE_F16)
+        fx_bounds_kernel<__half><<<grid, kFxThreads, 0, st>>>(attn, (const __half *)grad_out, row_map, qrows, na, ng, bounds);
     else if (grad_out_dtype == BEVF_DTYPE_F32)
         fx_bounds_kernel<float><<<grid, kFxThreads, 0, st>>>(attn, (const float *)grad_out, row_map, qrows, na, ng, bounds);
     else
@@ -110,6 +113,9 @@ extern "C" int bevf_msda_fx_convert(const int64_t *grad_value_fx, const uint32_t
     } else if (out_dtype == BEVF_DTYPE_BF16) {
         if (accumulate) fx_convert_kernel<bf16, true><<<grid, kFxThreads, 0, st>>>(fx, bounds, frac_bits, (bf16 *)out, n);
         else fx_convert_kernel<bf16, false><<<grid, kFxThreads, 0, st>>>(fx, bounds, frac_bits, (bf16 *)out, n);
+    } else if (out_dtype == BEVF_DTYPE_F16) {
+        if (accumulate) fx_convert_kernel<__half, true><<<grid, kFxThreads, 0, st>>>(fx, bounds, frac_bits, (__half *)out, n);
+        else fx_convert_kernel<__half, false><<<grid, kFxThreads, 0, st>>>(fx, bounds, frac_bits, (__half *)out, n);
     } else {
         return fail("%s: unsupported dtype code", who);
     }

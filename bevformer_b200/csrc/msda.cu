@@ -26,6 +26,7 @@
 
 #include <cstdlib>
 #include <cstring>
+#include <type_traits>
 
 #include "msda_common.cuh"
 
@@ -42,7 +43,7 @@ msda_fwd_d32(const T *__restrict__ value, const int64_t *__restrict__ level_hw,
              const int *__restrict__ row_map, int S, int M, int Q, int L, int P, int magic,
              int iters, long long rows) {
     constexpr int VEC = Vec<T>::N, LANES = 32 / VEC, G = 32 / LANES;
-    constexpr bool kHalf = (VEC == 8);
+    constexpr bool kHalf = std::is_same<T, bf16>::value;   // bf16: packed bf16 weights (fhfma); fp16: fp32 weights
     __shared__ LevelTab tab;
     load_level_tab(level_hw, level_start, L, M * 32, tab);
 
@@ -152,7 +153,7 @@ msda_bwd_d32(const T *__restrict__ value, const int64_t *__restrict__ level_hw,
     // red_skip: bit l set = the grad_value contributions of level l are NOT scattered here (hybrid mode: the
     // coarse levels go through msda_bwd_splat_d32, which merges them in registers, on a second stream)
     constexpr int VEC = Vec<T>::N, LANES = 32 / VEC, G = 32 / LANES;
-    constexpr bool kHalfDot = (VEC == 8) && (sizeof(TG) == 2);
+    constexpr bool kHalfDot = std::is_same<T, bf16>::value && std::is_same<TG, bf16>::value;
     __shared__ LevelTab tab;
     __shared__ unsigned s_skip;
     if (threadIdx.x == 0)     // levels masked for the dense path only if that kernel saw the same pyramid
@@ -626,12 +627,16 @@ static int launch_splat(const char *who, const float *loc, const float *attn, co
                         const int *row_map, const int *order, const int64_t *hw, const int64_t *ls,
                         int S, int M, int Q, int L, int P, long long pairs, unsigned level_mask,
                         cudaStream_t st) {
-    // the head count of every BEVFormer config is 8: that instance addresses the window with immediates
-    if (M == 8)
-        return launch_splat_km<TG, 8>(who, loc, attn, go, gv, row_map, order, hw, ls, S, M, Q, L, P, pairs,
+    if constexpr (std::is_same<TG, __half>::value) {
+        return fail("%s: the splat kernel takes fp32 or bf16 grad_out", who);
+    } else {
+        // the head count of every BEVFormer config is 8: that instance addresses the window with immediates
+        if (M == 8)
+            return launch_splat_km<TG, 8>(who, loc, attn, go, gv, row_map, order, hw, ls, S, M, Q, L, P, pairs,
+                                          level_mask, st);
+        return launch_splat_km<TG, 0>(who, loc, attn, go, gv, row_map, order, hw, ls, S, M, Q, L, P, pairs,
                                       level_mask, st);
-    return launch_splat_km<TG, 0>(who, loc, attn, go, gv, row_map, order, hw, ls, S, M, Q, L, P, pairs,
-                                  level_mask, st);
+    }
 }
 
 struct MixedGv {               // scaled-fp16 / mixed accumulation of grad_value (see msda_bwd_d32)
@@ -676,7 +681,7 @@ static int launch_bwd(const char *who, const void *value, const int64_t *hw, con
     }
     if (gv_f16) {
         // grad_value stored and accumulated in scaled fp16: bf16 value rows, head_dim 32, the one-kernel backward only
-        if constexpr (sizeof(T) == 2) {
+        if constexpr (std::is_same<T, bf16>::value) {
             if (D != 32) return fail("%s: fp16 grad_value needs head_dim 32", who);
             constexpr int G = Vec<T>::N;
             const int iters = pick_iters(rows, G);
@@ -692,7 +697,7 @@ static int launch_bwd(const char *who, const void *value, const int64_t *hw, con
         }
     }
     if (mixed && mixed->gv16) {
-        if constexpr (sizeof(T) == 2) {
+        if constexpr (std::is_same<T, bf16>::value) {
             if (D != 32) return fail("%s: mixed accumulation needs head_dim 32", who);
             constexpr int G = Vec<T>::N;
             const int iters = pick_iters(rows, G);
@@ -713,6 +718,8 @@ static int launch_bwd(const char *who, const void *value, const int64_t *hw, con
         const long long per_block = (long long)(kThreads / 32) * G * iters;
         const unsigned grid = (unsigned)((rows + per_block - 1) / per_block);
         const int mode = done_levels ? 0 : bwd_split_enabled();
+        if (mode != 0 && std::is_same<T, __half>::value)
+            return fail("%s: the split / hybrid backward modes take fp32 or bf16 only (fp16 needs mode 0)", who);
         const bool can_split = M <= kSplatMaxHeads && S * (long long)M * 32 < (1ll << 31);
         if (mode == 1 && can_split) {
             if (int e = launch_splat<TG>(who, loc, attn, go, gv, row_map, order, hw, ls, S, M, Q, L, P,
@@ -765,6 +772,12 @@ static int msda_forward_impl(const char *who, const void *value, int value_dtype
     if (!aligned16(value) || !aligned16(loc) || !aligned16(attn) || !aligned16(out))
         return fail("%s: device pointers must be 16-byte aligned", who);
     cudaStream_t st = (cudaStream_t)stream;
+    if (value_dtype == BEVF_DTYPE_F16) {
+        // fp16 value: fp16 or fp32 output
+        if (out_dtype == BEVF_DTYPE_F16) return launch_fwd<__half, __half>(who, value, level_hw, level_start, loc, attn, out, row_map, S, M, D, Q, L, P, rows, st);
+        if (out_dtype == BEVF_DTYPE_F32) return launch_fwd<__half, float>(who, value, level_hw, level_start, loc, attn, out, row_map, S, M, D, Q, L, P, rows, st);
+        return fail("%s: fp16 value needs an fp16 or fp32 output", who);
+    }
     const bool vb = value_dtype == BEVF_DTYPE_BF16, ob = out_dtype == BEVF_DTYPE_BF16;
     if ((value_dtype != BEVF_DTYPE_F32 && !vb) || (out_dtype != BEVF_DTYPE_F32 && !ob))
         return fail("%s: unsupported dtype code", who);
@@ -792,6 +805,12 @@ static int msda_backward_impl(const char *who, const void *value, int value_dtyp
         !aligned16(grad_value) || !aligned16(grad_loc) || !aligned16(grad_attn))
         return fail("%s: device pointers must be 16-byte aligned", who);
     cudaStream_t st = (cudaStream_t)stream;
+    if (value_dtype == BEVF_DTYPE_F16) {
+        // fp16 value: fp16 or fp32 grad_out; grad_value stays fp32 (or fixed point)
+        if (grad_out_dtype == BEVF_DTYPE_F16) return launch_bwd<__half, __half>(who, value, level_hw, level_start, loc, attn, grad_out, grad_value, grad_loc, grad_attn, row_map, order, S, M, D, Q, L, P, rows, st, done_levels, host_levels, gv_f16, mixed, fx);
+        if (grad_out_dtype == BEVF_DTYPE_F32) return launch_bwd<__half, float>(who, value, level_hw, level_start, loc, attn, grad_out, grad_value, grad_loc, grad_attn, row_map, order, S, M, D, Q, L, P, rows, st, done_levels, host_levels, gv_f16, mixed, fx);
+        return fail("%s: fp16 value needs an fp16 or fp32 grad_out", who);
+    }
     const bool vb = value_dtype == BEVF_DTYPE_BF16, gb = grad_out_dtype == BEVF_DTYPE_BF16;
     if ((value_dtype != BEVF_DTYPE_F32 && !vb) || (grad_out_dtype != BEVF_DTYPE_F32 && !gb))
         return fail("%s: unsupported dtype code", who);
@@ -900,6 +919,8 @@ extern "C" int bevf_msda_rows_backward_dense(const void *value, int value_dtype,
     memset(&hl, 0, sizeof(hl));
     const int mode = dense_mode();
     cudaEvent_t join = nullptr;
+    if (value_dtype == BEVF_DTYPE_F16 || grad_out_dtype == BEVF_DTYPE_F16)
+        return fail("%s: fp32 or bf16 only (fp16 runs on bevf_msda_rows_backward)", who);
     if (mode != 0 && D == 32 && grad_out_dtype == BEVF_DTYPE_BF16 && aligned16(loc) && aligned16(attn) &&
         aligned16(grad_out) && aligned16(grad_value)) {
         cudaStream_t ds = st;

@@ -157,6 +157,31 @@ template <> struct Vec<bf16> {
     }
 };
 
+// fp16 rows: widened exactly and multiplied with fp32 weights / gradients (no fp16 arithmetic)
+template <> struct Vec<__half> {
+    uint4 v;
+    static constexpr int N = 8;
+    __device__ __forceinline__ void load(const __half *p) { v = __ldg(reinterpret_cast<const uint4 *>(p)); }
+    __device__ __forceinline__ void axpy(float w, float (&acc)[8]) const {
+        const uint32_t u[4] = {v.x, v.y, v.z, v.w};
+#pragma unroll
+        for (int i = 0; i < 4; ++i) {
+            acc[2 * i] = fmaf(w, f16_lo(u[i]), acc[2 * i]);
+            acc[2 * i + 1] = fmaf(w, f16_hi(u[i]), acc[2 * i + 1]);
+        }
+    }
+    __device__ __forceinline__ float dot(const float (&g)[8]) const {
+        const uint32_t u[4] = {v.x, v.y, v.z, v.w};
+        float d = 0.f;
+#pragma unroll
+        for (int i = 0; i < 4; ++i) {
+            d = fmaf(g[2 * i], f16_lo(u[i]), d);
+            d = fmaf(g[2 * i + 1], f16_hi(u[i]), d);
+        }
+        return d;
+    }
+};
+
 template <int LANES> struct GroupMask;
 template <> struct GroupMask<4> { static constexpr unsigned kBits = 0x11111111u; };
 template <> struct GroupMask<8> { static constexpr unsigned kBits = 0x01010101u; };

@@ -334,6 +334,9 @@ extern "C" int bevf_msda_rows_forward_staged(const void *value, int value_dtype,
         cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
     }
     const int chunks = sms;                        // persistent: one CTA per SM
+    if ((value_dtype != BEVF_DTYPE_F32 && value_dtype != BEVF_DTYPE_BF16) ||
+        (out_dtype != BEVF_DTYPE_F32 && out_dtype != BEVF_DTYPE_BF16))
+        return fail("%s: fp32 or bf16 only (fp16 runs on bevf_msda_rows_forward)", who);
     const bool vb = value_dtype == BEVF_DTYPE_BF16, ob = out_dtype == BEVF_DTYPE_BF16;
     int e;
     if (vb && ob) e = launch_staged<bf16, bf16>(who, value, level_hw, level_start, level_hw_host, loc, attn, out, map_range, B, S, M, L, P, chunks, st);

@@ -15,8 +15,10 @@ from torch.autograd.function import Function, once_differentiable
 
 from . import _lib
 
-F32, BF16 = 0, 1
-_DT = {torch.float32: F32, torch.bfloat16: BF16}
+F32, BF16, F16 = 0, 1, 2
+_DT = {torch.float32: F32, torch.bfloat16: BF16, torch.float16: F16}
+# operand types of the tensor-core projections (fp32 accumulation for both)
+TC_DTYPES = (torch.bfloat16, torch.float16)
 
 
 def deterministic() -> bool:
@@ -99,7 +101,7 @@ def msda_forward(value, spatial_shapes, level_start_index, sampling_locations, a
                  out_dtype=None):
     """ms_deform_attn_forward: returns (B, Q, M*D) in ``out_dtype`` (default: value's dtype)."""
     if value.dtype not in _DT:
-        raise RuntimeError(f"value dtype {value.dtype} not supported (float32 or bfloat16)")
+        raise RuntimeError(f"value dtype {value.dtype} not supported (float32, bfloat16 or float16)")
     for t, n in ((value, "value"), (sampling_locations, "sampling_loc"),
                  (attention_weights, "attn_weight")):
         _need_cuda(t, n)
@@ -128,7 +130,7 @@ def msda_backward(value, spatial_shapes, level_start_index, sampling_locations, 
                  (attention_weights, "attn_weight"), (grad_output, "grad_output")):
         _need_cuda(t, n)
     if value.dtype not in _DT or grad_output.dtype not in _DT:
-        raise RuntimeError("value / grad_output must be float32 or bfloat16")
+        raise RuntimeError("value / grad_output must be float32, bfloat16 or float16")
     loc = sampling_locations if sampling_locations.dtype == torch.float32 else sampling_locations.float()
     attn = attention_weights if attention_weights.dtype == torch.float32 else attention_weights.float()
     B, S, M, D, Q, L, P = _dims(value, loc, attn)
@@ -193,8 +195,8 @@ def _cast_args(args, dtype):
 class MultiScaleDeformableAttnFunction_fp32(_MSDAFunction):
     """Same contract as the reference class of this name
     (multi_scale_deformable_attn_function.py:90-163): under autocast every floating input is cast
-    to fp32 first (``custom_fwd(cast_inputs=torch.float32)``, :93). Outside autocast a bf16 ``value``
-    is consumed natively (bf16 storage, fp32 accumulation) -- an extension the reference lacks."""
+    to fp32 first (``custom_fwd(cast_inputs=torch.float32)``, :93). Outside autocast a bf16 or fp16 ``value``
+    is consumed natively (16-bit storage, fp32 accumulation) -- an extension the reference lacks."""
 
     @staticmethod
     def forward(ctx, *args):
@@ -206,8 +208,9 @@ class MultiScaleDeformableAttnFunction_fp32(_MSDAFunction):
 
 class MultiScaleDeformableAttnFunction_fp16(_MSDAFunction):
     """Name kept for import compatibility (spatial_cross_attention.py:24-25, decoder.py:27-28).
-    The reference never selects it; half inputs are widened to fp32, the only half type the
-    library stores being bf16."""
+    The reference never selects it; as its ``custom_fwd(cast_inputs=torch.float32)`` does, every floating input
+    is widened to fp32 (this class keeps the reference contract; fp16 storage is reached through the _fp32 class
+    outside autocast or the plugin modules)."""
 
     @staticmethod
     def forward(ctx, *args):
@@ -227,7 +230,7 @@ def msda_rows_forward(value, spatial_shapes, level_start_index, loc, attn, row_m
     for t, n in ((value, "value"), (loc, "sampling_loc"), (attn, "attn_weight"), (row_map, "row_map")):
         _need_cuda(t, n)
     if value.dtype not in _DT or loc.dtype != torch.float32 or attn.dtype != torch.float32:
-        raise RuntimeError("value must be float32/bfloat16, sampling_loc and attn_weight float32")
+        raise RuntimeError("value must be float32/bfloat16/float16, sampling_loc and attn_weight float32")
     if row_map.dtype != torch.int32:
         raise RuntimeError("row_map must be int32")
     NB, S, M, D = value.shape
@@ -255,7 +258,7 @@ def msda_rows_forward_staged(value, spatial_shapes, level_start_index, level_hw_
     for t, n in ((value, "value"), (loc, "sampling_loc"), (attn, "attn_weight"), (map_range, "map_range")):
         _need_cuda(t, n)
     if value.dtype not in _DT or loc.dtype != torch.float32 or attn.dtype != torch.float32:
-        raise RuntimeError("value must be float32/bfloat16, sampling_loc and attn_weight float32")
+        raise RuntimeError("value must be float32/bfloat16/float16, sampling_loc and attn_weight float32")
     NB, S, M, D = value.shape
     R, M2, L, P, _ = loc.shape
     if M2 != M or tuple(attn.shape) != (R, M, L, P) or map_range.numel() != 2 * NB or len(level_hw_host) != L:
@@ -409,7 +412,7 @@ class FixedPointGradValue(LazyGradValue):
 
     def add_into(self, out: torch.Tensor) -> torch.Tensor:
         if out.dtype not in _DT or tuple(out.shape) != self.shape or not out.is_contiguous():
-            raise RuntimeError("add_into: a contiguous float32 / bfloat16 tensor of grad_value's shape is required")
+            raise RuntimeError("add_into: a contiguous float32 / bfloat16 / float16 tensor of grad_value's shape is required")
         return self._convert(out, True)
 
 
@@ -421,7 +424,7 @@ def msda_backward_fx(value, spatial_shapes, level_start_index, loc, attn, grad_o
     for t, n in ((value, "value"), (loc, "sampling_loc"), (attn, "attn_weight"), (grad_output, "grad_output")):
         _need_cuda(t, n)
     if value.dtype not in _DT or grad_output.dtype not in _DT:
-        raise RuntimeError("value / grad_output must be float32 or bfloat16")
+        raise RuntimeError("value / grad_output must be float32, bfloat16 or float16")
     loc = loc if loc.dtype == torch.float32 else loc.float()
     attn = attn if attn.dtype == torch.float32 else attn.float()
     NB, S, M, D = value.shape
@@ -554,11 +557,13 @@ class SamplerRows(Function):
     @staticmethod
     def forward(ctx, value, loc, attn, row_map, spatial_shapes, level_start_index, group_order=None,
                 staged=None, gv_mode=None):
-        """``staged`` = (level_hw_host, map_range): use the TMA-staged forward (rows grouped by value map)."""
-        if value.dtype == torch.float16:      # the reference widens half inputs (…function.py:93)
-            value = value.float()
+        """``staged`` = (level_hw_host, map_range): use the TMA-staged forward (rows grouped by value map).
+        An fp16 ``value`` is read natively (no widened copy); the staged, dense and fp16-accumulating variants take
+        bf16 / fp32 only and are skipped for it."""
+        half = value.dtype == torch.float16
         # an alternative to the plain kernel, opt-in for A/B runs
-        if staged is not None and value.shape[-1] == 32 and os.environ.get("BEVF_MSDA_FWD", "plain") == "staged":
+        if (staged is not None and not half and value.shape[-1] == 32
+                and os.environ.get("BEVF_MSDA_FWD", "plain") == "staged"):
             out = msda_rows_forward_staged(value, spatial_shapes, level_start_index, staged[0], loc, attn,
                                            staged[1])
         else:
@@ -568,7 +573,7 @@ class SamplerRows(Function):
         # grad_value accumulated in scaled fp16 -- "f16": every level, ("mixed", level_hw_host, n): the first n levels
         # -- (half the L2 reduction sectors of those levels): only where the caller asks for it
         ctx.gv_mode = gv_mode if (gv_mode is not None and value.dtype == torch.bfloat16 and value.shape[-1] == 32) else None
-        ctx.dense = staged if (staged is not None and value.shape[-1] == 32) else None
+        ctx.dense = staged if (staged is not None and not half and value.shape[-1] == 32) else None
         ctx.value_early = getattr(value, "_bevf_early", None)     # see plugin/linear.py::shared_input_projections
         ctx.gv_zero = None
         aux = aux_stream(value.device)
@@ -647,8 +652,8 @@ def sca_prep_forward(raw, ref_cam, pair_q, pair_cam, level_hw, B, Nq, M, L, P):
 
 def sca_prep_backward(raw, grad_loc, grad_attn, pair_of, level_hw, B, Nq, R, M, L, P,
                       out_dtype=torch.float32):
-    """d_raw of the SCA sampling-point prep; out_dtype=bfloat16 rounds in the kernel (the result then
-    feeds the bf16 GEMMs of the head without a cast pass)."""
+    """d_raw of the SCA sampling-point prep; out_dtype=bfloat16 / float16 rounds in the kernel (the result then
+    feeds the 16-bit GEMMs of the head without a cast pass)."""
     ncam = pair_of.shape[0]
     d_raw = torch.empty(raw.shape, device=raw.device, dtype=out_dtype)
     lib = _lib.load()
@@ -782,7 +787,7 @@ class LayerNormResidual(Function):
     def forward(ctx, x, residual, gamma, beta, eps, drop_p=0.0, pos=None, twin=False):
         _need_cuda(x, "x")
         if x.dtype not in _DT:
-            raise RuntimeError("layernorm: float32 or bfloat16 only")
+            raise RuntimeError("layernorm: float32, bfloat16 or float16 only")
         C = x.shape[-1]
         rows = x.numel() // C
         rc = None if residual is None else residual.contiguous()
@@ -956,34 +961,35 @@ def point_sampling(lidar2img, pc_range, z_norm, img_h, img_w, bev_h, bev_w, raw_
 
 
 def linear_tc(x, weight, bias=None, residual=None, relu=False, out_dtype=None):
-    """y = act(x @ weight.T + bias) (+ residual) on the wgmma GEMM.  x (..., K) bf16, weight (N, K)
-    bf16, bias (N) any float dtype, residual (..., N) bf16; returns (..., N) bf16 or fp32."""
+    """y = act(x @ weight.T + bias) (+ residual) on the wgmma GEMM.  x (..., K) and weight (N, K) both bf16 or
+    both fp16, bias (N) any float dtype, residual (..., N) in x's dtype; returns (..., N) in x's dtype (default)
+    or fp32."""
     _need_cuda(x, "x")
-    if x.dtype != torch.bfloat16 or weight.dtype != torch.bfloat16:
-        raise RuntimeError("linear_tc: x and weight must be bfloat16")
+    if x.dtype not in TC_DTYPES or weight.dtype != x.dtype:
+        raise RuntimeError("linear_tc: x and weight must be both bfloat16 or both float16")
     K = x.shape[-1]
     N = weight.shape[0]
     M = x.numel() // K
     w = weight.contiguous()
-    bq, bdt = (None, F32) if bias is None else _param_ptr(bias, torch.bfloat16)
+    bq, bdt = (None, F32) if bias is None else _param_ptr(bias, x.dtype)
     res = None if residual is None else residual.contiguous()
-    out_dtype = out_dtype or torch.bfloat16
+    out_dtype = out_dtype or x.dtype
     y = torch.empty(x.shape[:-1] + (N,), device=x.device, dtype=out_dtype)
     lib = _lib.load()
     with torch.cuda.device(x.device):
-        st = lib.bevf_linear_forward(x.data_ptr(), w.data_ptr(), _ptr(bq), bdt, _ptr(res), y.data_ptr(),
-                                     _DT[out_dtype], M, N, K, int(bool(relu)), _stream_ptr(x))
+        st = lib.bevf_linear_forward_dt(x.data_ptr(), w.data_ptr(), _ptr(bq), bdt, _ptr(res), y.data_ptr(),
+                                        _DT[out_dtype], M, N, K, int(bool(relu)), _DT[x.dtype], _stream_ptr(x))
     _lib.check(st, lib)
     return y
 
 
 def linear_dgrad_tc(dy, weight, addend=None):
     """dx = dy @ weight (+ addend) on the wgmma GEMM, the weight (N, K) read in place (no transposed
-    copy).  dy (M, N) bf16 -> (M, K) bf16; ``addend`` (M, K) bf16 is summed in the epilogue.  N or K not
-    a multiple of 64: falls back to the transposed-copy form."""
+    copy).  dy (M, N) bf16 / fp16 -> (M, K) of the same dtype; ``addend`` (M, K) of that dtype is summed in the
+    epilogue.  N or K not a multiple of 64: falls back to the transposed-copy form."""
     _need_cuda(dy, "dy")
-    if dy.dtype != torch.bfloat16 or weight.dtype != torch.bfloat16 or dy.shape[-1] != weight.shape[0]:
-        raise RuntimeError("linear_dgrad_tc: dy (M,N) and weight (N,K) must be bfloat16")
+    if dy.dtype not in TC_DTYPES or weight.dtype != dy.dtype or dy.shape[-1] != weight.shape[0]:
+        raise RuntimeError("linear_dgrad_tc: dy (M,N) and weight (N,K) must be both bfloat16 or both float16")
     N, K = weight.shape
     if N % 64 or K % 64 or os.environ.get("BEVF_DGRAD", "mn") == "copy":
         dx = linear_tc(dy, weight.t().contiguous())
@@ -991,28 +997,29 @@ def linear_dgrad_tc(dy, weight, addend=None):
     dy = dy.contiguous()
     w = weight.contiguous()
     M = dy.numel() // N
-    dx = torch.empty(dy.shape[:-1] + (K,), device=dy.device, dtype=torch.bfloat16)
+    dx = torch.empty(dy.shape[:-1] + (K,), device=dy.device, dtype=dy.dtype)
     lib = _lib.load()
     with torch.cuda.device(dy.device):
         if addend is None:
-            st = lib.bevf_linear_dgrad(dy.data_ptr(), w.data_ptr(), dx.data_ptr(), M, N, K, _stream_ptr(dy))
+            st = lib.bevf_linear_dgrad_dt(dy.data_ptr(), w.data_ptr(), dx.data_ptr(), M, N, K, _DT[dy.dtype],
+                                          _stream_ptr(dy))
         else:
-            if addend.dtype != torch.bfloat16 or addend.numel() != M * K or not addend.is_contiguous():
-                raise RuntimeError("linear_dgrad_tc: addend must be a contiguous bf16 (M, K) tensor")
-            st = lib.bevf_linear_dgrad_acc(dy.data_ptr(), w.data_ptr(), addend.data_ptr(), dx.data_ptr(), M, N, K,
-                                           _stream_ptr(dy))
+            if addend.dtype != dy.dtype or addend.numel() != M * K or not addend.is_contiguous():
+                raise RuntimeError("linear_dgrad_tc: addend must be a contiguous (M, K) tensor of dy's dtype")
+            st = lib.bevf_linear_dgrad_acc_dt(dy.data_ptr(), w.data_ptr(), addend.data_ptr(), dx.data_ptr(), M, N, K,
+                                              _DT[dy.dtype], _stream_ptr(dy))
     _lib.check(st, lib)
     return dx
 
 
 def linear_wgrad_tc(dy, x, with_bias=False, out_dtype=None):
     """dW = dy^T @ x on the wgmma split-M kernel (and db = column sums of dy from the same pass).
-    dy (M, N) bf16, x (M, K) bf16 -> (N, K) fp32 [, (N,) fp32].  The kernel accumulates in one fp32
+    dy (M, N), x (M, K) both bf16 or both fp16 -> (N, K) fp32 [, (N,) fp32].  The kernel accumulates in one fp32
     buffer holding [dW | db]; ``out_dtype`` converts that buffer once (dW and db are views of it)."""
     _need_cuda(dy, "dy")
     _need_cuda(x, "x")
-    if dy.dtype != torch.bfloat16 or x.dtype != torch.bfloat16 or dy.shape[0] != x.shape[0]:
-        raise RuntimeError("linear_wgrad_tc: dy (M,N) and x (M,K) must be bfloat16 with equal M")
+    if dy.dtype not in TC_DTYPES or x.dtype != dy.dtype or dy.shape[0] != x.shape[0]:
+        raise RuntimeError("linear_wgrad_tc: dy (M,N) and x (M,K) must be both bfloat16 or both float16 with equal M")
     M, N = dy.shape
     K = x.shape[1]
     npad = (N + 3) // 4 * 4
@@ -1032,8 +1039,8 @@ def linear_wgrad_into(dy, x, dw_acc, db_acc=None):
     gradient arena): no allocation, no zero-fill, no conversion here."""
     _need_cuda(dy, "dy")
     _need_cuda(x, "x")
-    if dy.dtype != torch.bfloat16 or x.dtype != torch.bfloat16 or dy.shape[0] != x.shape[0]:
-        raise RuntimeError("linear_wgrad_into: dy (M,N) and x (M,K) must be bfloat16 with equal M")
+    if dy.dtype not in TC_DTYPES or x.dtype != dy.dtype or dy.shape[0] != x.shape[0]:
+        raise RuntimeError("linear_wgrad_into: dy (M,N) and x (M,K) must be both bfloat16 or both float16 with equal M")
     M, N = dy.shape
     K = x.shape[1]
     if dw_acc.dtype != torch.float32 or dw_acc.numel() != N * K or not dw_acc.is_contiguous():
@@ -1051,10 +1058,11 @@ def _wgrad_acc(dy, x, dw, db):
         if deterministic() and M > 0:
             need = int(lib.bevf_linear_wgrad_workspace_bytes(M, N, K))
             ws = torch.empty(need, device=x.device, dtype=torch.uint8)
-            st = lib.bevf_linear_wgrad_into(dy.data_ptr(), x.data_ptr(), dw.data_ptr(), _ptr(db), ws.data_ptr(), need,
-                                            M, N, K, _stream_ptr(x))
+            st = lib.bevf_linear_wgrad_into_dt(dy.data_ptr(), x.data_ptr(), dw.data_ptr(), _ptr(db), ws.data_ptr(),
+                                               need, M, N, K, _DT[x.dtype], _stream_ptr(x))
         else:
-            st = lib.bevf_linear_wgrad(dy.data_ptr(), x.data_ptr(), dw.data_ptr(), _ptr(db), M, N, K, _stream_ptr(x))
+            st = lib.bevf_linear_wgrad_dt(dy.data_ptr(), x.data_ptr(), dw.data_ptr(), _ptr(db), M, N, K, _DT[x.dtype],
+                                          _stream_ptr(x))
     _lib.check(st, lib)
 
 
@@ -1062,8 +1070,8 @@ def linear_wgrad_out(dy, x, grad_dtype, with_bias):
     """Two-pass weight (+ bias) gradient written directly in ``grad_dtype``: returns (dW, db|None)."""
     _need_cuda(dy, "dy")
     _need_cuda(x, "x")
-    if dy.dtype != torch.bfloat16 or x.dtype != torch.bfloat16 or dy.shape[0] != x.shape[0]:
-        raise RuntimeError("linear_wgrad_out: dy (M,N) and x (M,K) must be bfloat16 with equal M")
+    if dy.dtype not in TC_DTYPES or x.dtype != dy.dtype or dy.shape[0] != x.shape[0]:
+        raise RuntimeError("linear_wgrad_out: dy (M,N) and x (M,K) must be both bfloat16 or both float16 with equal M")
     M, N = dy.shape
     K = x.shape[1]
     lib = _lib.load()
@@ -1072,8 +1080,8 @@ def linear_wgrad_out(dy, x, grad_dtype, with_bias):
         ws = torch.empty(need, device=x.device, dtype=torch.uint8)
         dw = torch.empty((N, K), device=x.device, dtype=grad_dtype)
         db = torch.empty((N,), device=x.device, dtype=grad_dtype) if with_bias else None
-        st = lib.bevf_linear_wgrad_out(dy.data_ptr(), x.data_ptr(), dw.data_ptr(), _ptr(db),
-                                       _DT[grad_dtype], ws.data_ptr(), need, M, N, K, _stream_ptr(x))
+        st = lib.bevf_linear_wgrad_out_dt(dy.data_ptr(), x.data_ptr(), dw.data_ptr(), _ptr(db),
+                                          _DT[grad_dtype], ws.data_ptr(), need, M, N, K, _DT[x.dtype], _stream_ptr(x))
     _lib.check(st, lib)
     return dw, db
 
@@ -1087,7 +1095,7 @@ def sum_tensors(ts):
     t0 = ts[0]
     _need_cuda(t0, "tensors[0]")
     if len(ts) > 8 or any(t.shape != t0.shape or t.dtype != t0.dtype for t in ts) or t0.dtype not in _DT:
-        raise RuntimeError("sum_tensors: 1..8 tensors of one shape, float32 or bfloat16")
+        raise RuntimeError("sum_tensors: 1..8 tensors of one shape, float32, bfloat16 or float16")
     out = torch.empty_like(t0)
     arr = (ctypes.c_void_p * len(ts))(*[t.data_ptr() for t in ts])
     lib = _lib.load()
@@ -1154,7 +1162,7 @@ class FlattenFeats(Function):
         f0 = feats[0]
         _need_cuda(f0, "mlvl_feats[0]")
         if f0.dtype not in _DT:
-            raise RuntimeError("flatten_feats: float32 or bfloat16 only")
+            raise RuntimeError("flatten_feats: float32, bfloat16 or float16 only")
         bs, ncam, C = f0.shape[:3]
         hws = [int(f.shape[3] * f.shape[4]) for f in feats]
         S = sum(hws)

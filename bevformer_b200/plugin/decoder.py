@@ -21,7 +21,7 @@ import torch.nn as nn
 
 import copy
 
-from .. import ops
+from .. import ops, precision
 from .linear import linear, linear_fp32_out
 from .registry import (ATTENTION, HAVE_MMCV, TRANSFORMER_LAYER, TRANSFORMER_LAYER_SEQUENCE, _register,
                        build_transformer_layer)
@@ -60,6 +60,7 @@ class CustomMSDeformableAttention(nn.Module):
             nn.init.zeros_(lin.bias)
         self._is_init = True
 
+    @precision.entry("query", "key", "value", "identity", "query_pos")
     def forward(self, query, key=None, value=None, identity=None, query_pos=None,
                 key_padding_mask=None, reference_points=None, spatial_shapes=None,
                 level_start_index=None, flag="decoder", **kwargs):

@@ -23,7 +23,7 @@ import numpy as np
 import torch
 import torch.nn as nn
 
-from .. import ops
+from .. import ops, precision
 from .linear import linear, linear_relu_dropout, shared_input_projections
 from .registry import (FEEDFORWARD_NETWORK, HAVE_MMCV, TRANSFORMER_LAYER, TRANSFORMER_LAYER_SEQUENCE, _register,
                        build_attention, build_feedforward_network, build_transformer_layer)
@@ -99,6 +99,7 @@ class FFN(nn.Module):
         last = self.layers[self.num_fcs - 1]
         return linear(h, last.weight, last.bias)
 
+    @precision.entry("x", "identity")
     def forward(self, x, identity=None):
         out = self.layers[self.num_fcs](self.transform(x))
         if not self.add_identity:
@@ -119,10 +120,9 @@ def _fused_norm(norm: nn.LayerNorm, x, residual, dropout: Optional[nn.Dropout] =
     that produced x is applied inside, active only in training mode).  With ``pos`` the kernel also
     emits y + pos and the call returns (y, y + pos); with ``twin`` it returns (y, alias of y) so that the
     next block and its residual connection receive separate gradients (summed inside the backward kernel
-    instead of by autograd).  Shapes / dtypes the kernel does not cover
-    (fp16 activations under the reference's fp16 configs, embed_dims other than 256 / 512) take the
+    instead of by autograd).  Shapes the kernel does not cover (embed_dims other than 256 / 512) take the
     unfused CUDA ops instead."""
-    if x.dtype not in (torch.float32, torch.bfloat16) or x.shape[-1] not in (256, 512):
+    if x.dtype not in (torch.float32, torch.bfloat16, torch.float16) or x.shape[-1] not in (256, 512):
         h = x if dropout is None else dropout(x)
         y = norm(h if residual is None else h + residual)
         if pos is None and twin:
@@ -557,12 +557,14 @@ class BEVFormerEncoder(nn.Module):
         return cache[key]
 
     # ---- forward ---------------------------------------------------------------------------------
+    @precision.entry("bev_query", "key", "value", "bev_pos", "prev_bev")
     def forward(self, bev_query, key, value, *args, bev_h=None, bev_w=None, bev_pos=None,
                 spatial_shapes=None, level_start_index=None, valid_ratios=None, prev_bev=None,
                 shift=0.0, **kwargs):
         """bev_query / bev_pos / prev_bev (Nq, bs, C); key = value (num_cams, S, bs, C);
         returns (bs, Nq, C), or (num_layers, bs, Nq, C) with return_intermediate
-        (same contract as encoder.py:151-239)."""
+        (same contract as encoder.py:151-239).  Under autocast, or with ``fp16_enabled``, the activations are
+        cast once to the compute dtype (bevformer_b200.precision) and the result is returned in it."""
         bs = bev_query.size(1)
         dev, dtype = bev_query.device, bev_query.dtype
         ref_2d, tsa_ss, tsa_lsi = self._constants(bev_h, bev_w, bs, dev)
@@ -600,7 +602,7 @@ class BEVFormerEncoder(nn.Module):
         fusable = [l for l in self.layers if isinstance(l, BEVFormerLayer) and not l.pre_norm
                    and len(l.attentions) == 2 and isinstance(l.attentions[0], TemporalSelfAttention)
                    and isinstance(l.attentions[1], SpatialCrossAttention)]
-        if (len(fusable) == len(self.layers) and dev.type == "cuda" and dtype == torch.bfloat16
+        if (len(fusable) == len(self.layers) and dev.type == "cuda" and dtype in ops.TC_DTYPES
                 and key_padding_free(kwargs) and value is not None):
             ncam, s_len, c = value.shape[0], value.shape[1], value.shape[3]
             feats = value.permute(2, 0, 1, 3).reshape(bs * ncam, s_len, c)

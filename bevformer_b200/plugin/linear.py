@@ -1,7 +1,7 @@
 """The dense projections of the encoder layer (value_proj / output_proj / the stacked
 sampling_offsets|attention_weights head / FFN) behind one function.
 
-bf16 CUDA inputs run on the hand-written wgmma kernel of ``csrc/gemm.cu`` (bias, ReLU and the fp32
+bf16 / fp16 CUDA inputs run on the hand-written wgmma kernel of ``csrc/gemm.cu`` (bias, ReLU and the fp32
 result of the offsets|logits head fused into its epilogue); its backward uses the same kernel for
 dX = dY . W and the split-M wgmma kernel for dW = dY^T . X (``BEVF_WGRAD=cublas`` switches that one
 back to the library); bias gradients come from the column-sum kernel.
@@ -21,7 +21,7 @@ from ..arena import arena_of
 
 
 def _use_tc(x: torch.Tensor, weight: torch.Tensor) -> bool:
-    return (x.is_cuda and x.dtype == torch.bfloat16 and weight.shape[1] % 64 == 0
+    return (x.is_cuda and x.dtype in ops.TC_DTYPES and weight.shape[1] % 64 == 0
             and weight.shape[0] % 16 == 0 and os.environ.get("BEVF_GEMM", "tc") != "cublas")
 
 
@@ -30,7 +30,7 @@ def stacked_head(weights, biases, x):
     On the wgmma path with a gradient arena the stack is a view of the arena's parameter buffer."""
     from ..arena import stacked
     n, k = sum(w.shape[0] for w in weights), weights[0].shape[1]
-    direct = (x.is_cuda and x.dtype == torch.bfloat16 and k % 64 == 0 and n % 16 == 0
+    direct = (x.is_cuda and x.dtype in ops.TC_DTYPES and k % 64 == 0 and n % 16 == 0
               and os.environ.get("BEVF_GEMM", "tc") != "cublas")
     return stacked(weights, direct), stacked(biases, direct)
 
@@ -44,9 +44,9 @@ def _arena_ctx(weight, bias):
 class _LinearTC(Function):
     @staticmethod
     def forward(ctx, x, weight, bias, relu, fp32_out):
-        w = weight.to(torch.bfloat16)
+        w = weight.to(x.dtype)           # weights run in the activation dtype (a cast per call for fp32 masters)
         xc = x.contiguous()
-        y = ops.linear_tc(xc, w, bias, None, relu, torch.float32 if fp32_out else torch.bfloat16)
+        y = ops.linear_tc(xc, w, bias, None, relu, torch.float32 if fp32_out else x.dtype)
         ctx.save_for_backward(xc, w, y if relu else None)
         ctx.has_bias = bias is not None
         ctx.dtypes = (weight.dtype, None if bias is None else bias.dtype)
@@ -61,7 +61,7 @@ class _LinearTC(Function):
         dy2 = dy.reshape(-1, n)
         if y is not None:                                  # ReLU: gradient only where the output is > 0
             dy2 = dy2 * (y.reshape(-1, n) > 0)
-        dy2 = dy2.to(torch.bfloat16).contiguous()
+        dy2 = dy2.to(w.dtype).contiguous()
         dx = dw = db = None
         if ctx.needs_input_grad[0]:
             dx = ops.linear_dgrad_tc(dy2, w).view(x.shape)
@@ -85,7 +85,7 @@ def _wgrad(dy2, x2, n, k, wdtype, bdtype=None, arena=None):
         ar.run_off_critical_path(lambda: ops.linear_wgrad_into(dy2, x2, dw_acc, db_acc), dy2, x2)
         return None, None
     mode = os.environ.get("BEVF_WGRAD", "tc")     # "tc2": two-pass variant (opt-in)
-    if mode == "tc2" and n % 8 == 0 and wdtype in (torch.bfloat16, torch.float32) and bdtype in (None, wdtype):
+    if mode == "tc2" and n % 8 == 0 and wdtype in (torch.bfloat16, torch.float16, torch.float32) and bdtype in (None, wdtype):
         return ops.linear_wgrad_out(dy2, x2, wdtype, bdtype is not None)
     if mode != "cublas" and n % 8 == 0:
         if bdtype is None:
@@ -104,9 +104,9 @@ class _LinearReluDropoutTC(Function):
 
     @staticmethod
     def forward(ctx, x, weight, bias, p):
-        w = weight.to(torch.bfloat16)
+        w = weight.to(x.dtype)
         xc = x.contiguous()
-        h = ops.linear_tc(xc, w, bias, None, True, torch.bfloat16)
+        h = ops.linear_tc(xc, w, bias, None, True, x.dtype)
         ops.dropout_inplace_(h, p)
         ctx.save_for_backward(xc, w, h)
         ctx.meta = (bias is not None, weight.dtype, None if bias is None else bias.dtype, float(p))
@@ -154,13 +154,13 @@ class _SharedInputProjections(Function):
             ev.record(main)
             aux.wait_event(ev)
         for i in range(0, len(wb), 2):
-            w = wb[i].to(torch.bfloat16)
+            w = wb[i].to(xc.dtype)
             ws.append(w)
             if aux is None:
-                outs.append(ops.linear_tc(xc, w, wb[i + 1], None, False, torch.bfloat16))
+                outs.append(ops.linear_tc(xc, w, wb[i + 1], None, False, xc.dtype))
             else:
                 with torch.cuda.stream(aux):
-                    o = ops.linear_tc(xc, w, wb[i + 1], None, False, torch.bfloat16)
+                    o = ops.linear_tc(xc, w, wb[i + 1], None, False, xc.dtype)
                     e = torch.cuda.Event()
                     e.record(aux)
                 o.record_stream(main)
@@ -198,9 +198,9 @@ class _SharedInputProjections(Function):
         box = {}
 
         def work():
-            # (the fp32 -> bf16 conversion of a sampler's grad_value happens here too, off the critical path)
+            # (the fp32 -> bf16 / fp16 conversion of a sampler's grad_value happens here too, off the critical path)
             dyt = dy.materialize() if isinstance(dy, ops.LazyGradValue) else dy    # fp16 accumulators -> bf16 here
-            dy2 = dyt.reshape(-1, n).to(torch.bfloat16).contiguous()
+            dy2 = dyt.reshape(-1, n).to(w.dtype).contiguous()
             if state["need_dx"]:
                 box["dx"] = ops.linear_dgrad_tc(dy2, w)
             dw_acc, db_acc = ar[1][0].view(n, k), (ar[1][1] if len(ar[1]) > 1 else None)
@@ -236,7 +236,7 @@ class _SharedInputProjections(Function):
                     dxs.append(box["dx"])
                 grads += [None, None]
                 continue
-            dy2 = dy.reshape(-1, n).to(torch.bfloat16).contiguous()
+            dy2 = dy.reshape(-1, n).to(w.dtype).contiguous()
             if ctx.needs_input_grad[1]:
                 dxs.append(ops.linear_dgrad_tc(dy2, w))
             dw = db = None
@@ -306,7 +306,7 @@ def linear_fp32_out(x: torch.Tensor, weight: torch.Tensor, bias) -> torch.Tensor
 class _HeadTC(Function):
     @staticmethod
     def forward(ctx, x, weight, bias, kind, prep_args):
-        w = weight.to(torch.bfloat16)
+        w = weight.to(x.dtype)
         xc = x.contiguous()
         raw = ops.linear_tc(xc, w, bias, None, False, torch.float32).reshape(-1, w.shape[0])
         if kind == "sca":
@@ -331,11 +331,11 @@ class _HeadTC(Function):
         if ctx.kind == "sca":
             _ref_cam, pair_q, _pair_cam, pair_of, ss, bs, nq, m, l, p = ctx.prep_args
             d_raw = ops.sca_prep_backward(raw, grad_loc, grad_attn, pair_of, ss, bs, nq,
-                                          pair_q.numel(), m, l, p, out_dtype=torch.bfloat16)
+                                          pair_q.numel(), m, l, p, out_dtype=w.dtype)
         else:
             _ref, ss, bs, nq, m, l, p, interleave = ctx.prep_args
             d_raw = ops.tsa_prep_backward(raw, grad_loc, grad_attn, ss, bs, nq, m, l, p, interleave,
-                                          out_dtype=torch.bfloat16)
+                                          out_dtype=w.dtype)
         dx = dw = db = None
         if ctx.needs_input_grad[0]:
             dx = ops.linear_dgrad_tc(d_raw, w).view(x.shape)

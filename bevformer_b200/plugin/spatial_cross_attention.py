@@ -21,7 +21,7 @@ from typing import Optional
 import torch
 import torch.nn as nn
 
-from .. import ops
+from .. import ops, precision
 from .linear import linear, sca_sampling_head, stacked_head
 from .registry import ATTENTION, _register, build_attention
 from .temporal_self_attention import _check_head_dim, ring_offsets_
@@ -139,6 +139,7 @@ class MSDeformableAttention3D(nn.Module):
                   (self.sampling_offsets.bias, self.attention_weights.bias)
         return stacked_head(ws, bs_, x)
 
+    @precision.entry("query", "key", "value", "identity", "query_pos")
     def forward(self, query, key=None, value=None, identity=None, query_pos=None,
                 key_padding_mask=None, reference_points=None, spatial_shapes=None,
                 level_start_index=None, **kwargs):
@@ -245,6 +246,7 @@ class SpatialCrossAttention(nn.Module):
         slots = ops.ScaCombine.apply(out, plan.pair_of, plan.pair_q, plan.inv_count, bs, nq)
         return linear(slots, self.output_proj.weight, self.output_proj.bias)
 
+    @precision.entry("query", "key", "value", "residual", "query_pos")
     def forward(self, query, key, value, residual=None, query_pos=None, key_padding_mask=None,
                 reference_points=None, spatial_shapes=None, reference_points_cam=None,
                 bev_mask=None, level_start_index=None, flag="encoder", **kwargs):

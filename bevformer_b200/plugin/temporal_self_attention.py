@@ -16,7 +16,7 @@ import warnings
 import torch
 import torch.nn as nn
 
-from .. import ops
+from .. import ops, precision
 from .linear import linear, linear_fp32_out, stacked_head, tsa_sampling_head
 from .registry import ATTENTION, _register
 
@@ -194,6 +194,7 @@ class TemporalSelfAttention(nn.Module):
         loc = rp[:, :, None, :, None, :2] + off / p * rp[:, :, None, :, None, 2:] * 0.5
         return loc.contiguous(), att
 
+    @precision.entry("query", "key", "value", "identity", "query_pos")
     def forward(self, query, key=None, value=None, identity=None, query_pos=None,
                 key_padding_mask=None, reference_points=None, spatial_shapes=None,
                 level_start_index=None, flag="decoder", **kwargs):

@@ -18,7 +18,7 @@ import numpy as np
 import torch
 import torch.nn as nn
 
-from .. import ops
+from .. import ops, precision
 from .registry import TRANSFORMER, _register, build_transformer_layer_sequence
 
 
@@ -106,7 +106,15 @@ class PerceptionTransformer(nn.Module):
                          bev_pos=None, prev_bev=None, **kwargs):
         """mlvl_feats: per level (bs, num_cams, C, h, w); bev_queries (Nq, C); bev_pos
         (bs, C, bev_h, bev_w); prev_bev (bs, Nq, C) / (Nq, bs, C) / None; kwargs carry ``img_metas``.
-        Returns bev_embed (bs, Nq, C)."""
+        Returns bev_embed (bs, Nq, C) in the compute dtype: the autocast dtype, fp16 with ``fp16_enabled``
+        (what mmcv's auto_fp16 gives), else the features' dtype (bevformer_b200.precision)."""
+        dt, amp_off = precision.entered(self, mlvl_feats[0])
+        with amp_off:
+            return self._get_bev_features(precision.cast(list(mlvl_feats), dt), bev_queries, bev_h, bev_w, dt,
+                                          grid_length, bev_pos, prev_bev, **kwargs)
+
+    def _get_bev_features(self, mlvl_feats, bev_queries, bev_h, bev_w, dt, grid_length, bev_pos, prev_bev,
+                          **kwargs):
         img_metas = kwargs["img_metas"]
         bs = mlvl_feats[0].size(0)
         bev_queries = bev_queries.unsqueeze(1).repeat(1, bs, 1)
@@ -120,6 +128,8 @@ class PerceptionTransformer(nn.Module):
         can_bus = bev_queries.new_tensor([m["can_bus"] for m in img_metas])
         can_bus = self.can_bus_mlp(can_bus)[None, :, :]
         bev_queries = bev_queries + can_bus * self.use_can_bus
+        # (the can_bus MLP above runs in its parameters' dtype; the encoder from here on in the compute dtype)
+        bev_queries, bev_pos, prev_bev = (precision.cast(t, dt) for t in (bev_queries, bev_pos, prev_bev))
 
         shapes = [tuple(f.shape[-2:]) for f in mlvl_feats]
         if mlvl_feats[0].is_cuda:
@@ -177,10 +187,12 @@ class PerceptionTransformerBEVEncoder(nn.Module):
         if self.use_cams_embeds:
             nn.init.normal_(self.cams_embeds)
 
+    @precision.entry("mlvl_feats", "bev_queries", "bev_pos")
     def forward(self, mlvl_feats, bev_queries, bev_h, bev_w, grid_length=[0.512, 0.512], bev_pos=None,
                 prev_bev=None, **kwargs):
-        """Returns the BEV features (bs, bev_h*bev_w, C); ``prev_bev`` is accepted and ignored, as in
-        the reference (:97-141)."""
+        """Returns the BEV features (bs, bev_h*bev_w, C) in the compute dtype (bevformer_b200.precision);
+        ``prev_bev`` is accepted and ignored, as in the reference (:97-141).  Also the encoder half of
+        PerceptionTransformerV2."""
         if not mlvl_feats[0].is_cuda:
             raise RuntimeError("PerceptionTransformerBEVEncoder: CUDA tensors required "
                                "(bevformer_b200 has no CPU path)")
@@ -349,7 +361,7 @@ def patch_reference(cls):
     (which keeps its decoder ``forward``): ``patch_reference(PerceptionTransformer)`` once at import
     time of a BEVFormer checkout.  Parameter / attribute names are the reference's, so nothing else
     changes; the encoder inside is whatever the config built (the drop-in BEVFormerEncoder)."""
-    for name in ("get_bev_features", "_shift", "_rotate_prev"):
+    for name in ("get_bev_features", "_get_bev_features", "_shift", "_rotate_prev"):
         setattr(cls, name, getattr(PerceptionTransformer, name))
     return cls
 

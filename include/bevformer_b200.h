@@ -46,7 +46,9 @@ extern "C" {
 #define BEVF_API
 #endif
 
-enum bevf_dtype { BEVF_DTYPE_F32 = 0, BEVF_DTYPE_BF16 = 1 };
+/* Storage types.  fp16 stores round to nearest and overflow to +-inf (never saturate), so loss scaling sees the
+ * overflow; every kernel widens 16-bit inputs exactly and accumulates in fp32. */
+enum bevf_dtype { BEVF_DTYPE_F32 = 0, BEVF_DTYPE_BF16 = 1, BEVF_DTYPE_F16 = 2 };
 
 /* ABI version of the loaded library (== BEVF_ABI_VERSION it was built with). */
 BEVF_API int bevf_version(void);
@@ -65,12 +67,13 @@ BEVF_API int64_t bevf_launch_count(void);
  *   multi_scale_deformable_attn_function.py:118-124 (from temporal_self_attention.py:247,
  *   spatial_cross_attention.py:390, decoder.py:332).
  *
- *   value        (B, S, M, D)        value_dtype (f32 | bf16)
+ *   value        (B, S, M, D)        value_dtype (f32 | bf16 | f16)
  *   level_hw     (L, 2) int64 DEVICE (h, w) per level          -- the reference's spatial_shapes
  *   level_start  (L,)   int64 DEVICE first row of each level   -- the reference's level_start_index
  *   loc          (B, Q, M, L, P, 2) f32, (x, y) normalised to [0,1] over each level
  *   attn         (B, Q, M, L, P)    f32
- *   out          (B, Q, M*D)        out_dtype (f32 | bf16), fully overwritten
+ *   out          (B, Q, M*D)        out_dtype (f32 | bf16 | f16), fully overwritten; a 16-bit out
+ *                                   needs the same value dtype (bf16 value may write f32, f16 value f32)
  *
  * out[b,q,m,:] = sum_l sum_p attn * bilinear(value_l, x = loc_x*W_l - 0.5, y = loc_y*H_l - 0.5),
  * zero padding, a sample contributes only if -1 < x < W_l and -1 < y < H_l (SURVEY.md Appendix A).
@@ -85,7 +88,7 @@ BEVF_API int bevf_msda_forward(const void *value, int value_dtype, const int64_t
  * replaces: mmcv._ext.ms_deform_attn_backward, as called at
  *   multi_scale_deformable_attn_function.py:150-160.
  *
- *   grad_out    (B, Q, M*D)  grad_out_dtype (f32 | bf16)
+ *   grad_out    (B, Q, M*D)  grad_out_dtype (f32 | bf16 | f16; a 16-bit grad_out matches value_dtype)
  *   grad_value  (B, S, M, D) f32 -- ACCUMULATED INTO (caller zero-fills, as the reference does at
  *                                   multi_scale_deformable_attn_function.py:146)
  *   grad_loc    (B, Q, M, L, P, 2) f32 -- fully overwritten (zeros for skipped samples)
@@ -160,7 +163,8 @@ BEVF_API int bevf_msda_rows_backward_ordered(const void *value, int value_dtype,
  *                                             levels lie before / after it from the DEVICE pyramid (a device level
  *                                             that straddles S_fine is a caller bug and traps)
  *   bevf_gv_merge(fine, side, amax, out, B, S, S_fine, row_elems)   out (B, S, row_elems) bf16 from both
- * All need a bf16 value tensor and head_dim 32; grad_loc / grad_attn are those of the fp32 path bit for bit.
+ * All need a bf16 value tensor and head_dim 32 (fp16 value is an error); grad_loc / grad_attn are those of the fp32
+ * path bit for bit.
  */
 BEVF_API int bevf_abs_max(const void *x, int dtype, int64_t n, uint32_t *amax_bits, void *stream);
 BEVF_API int bevf_msda_rows_backward_f16acc(const void *value, int value_dtype, const int64_t *level_hw,
@@ -194,7 +198,7 @@ BEVF_API int bevf_gv_merge(const void *fine_f16, const float *side_f32, const ui
  *       bounds         2 uint32 DEVICE words, written: the bits of max|attn| and max|grad_out| over the launch's rows
  *                      (rows with row_map < 0 excluded), sign cleared; the conversion reads them
  *       frac_bits      K, at most bevf_msda_fx_frac_bits(Q or R, L, P)
- *   bevf_msda_fx_convert(fx, bounds, K, out, out_dtype, accumulate, n)   out (f32 | bf16) = fx * 2^(E - K), or
+ *   bevf_msda_fx_convert(fx, bounds, K, out, out_dtype, accumulate, n)   out (f32 | bf16 | f16) = fx * 2^(E - K), or
  *                                                out += that with accumulate != 0 (bevf_msda_backward's contract)
  * Scale: E = (floor(log2 max|attn|) + 1) + (floor(log2 max|grad_out|) + 1), so every contribution w * attn * g
  * (w <= 1) is below 2^E.  A contribution is formed exactly (the fp32 products w * attn and (w * attn) * g in double),
@@ -229,7 +233,7 @@ BEVF_API int bevf_msda_fx_convert(const int64_t *grad_value_fx, const uint32_t *
  *                  whose host shape disagrees with the device-side level_hw / level_start is not staged
  *   map_range      (B, 2) int32 DEVICE: [first, end) rows of every value map (bevf_sca_plan_build)
  *   B = number of value maps; levels must be stored back to back (level_start[l] = sum of H*W before l,
- *   the reference's own definition, transformer.py:178-180); head_dim 32.
+ *   the reference's own definition, transformer.py:178-180); head_dim 32; fp32 or bf16 only (fp16 is an error).
  */
 BEVF_API int bevf_msda_rows_forward_staged(const void *value, int value_dtype, const int64_t *level_hw,
                                            const int64_t *level_start, const int32_t *level_hw_host,
@@ -247,7 +251,8 @@ BEVF_API int bevf_msda_rows_forward_staged(const void *value, int value_dtype, c
  * by one thread per (row, level) and multiplied with wgmma.  Levels with more than BEVF_DENSE_MAXPIX
  * pixels (default 8192), grad_loc and grad_attn come from the one-kernel backward as before.
  * Used when grad_out is bf16 and head_dim is 32 with 4 or 8 points per level; any other configuration
- * runs exactly bevf_msda_rows_backward.  grad_value must be zero-filled or hold a running sum, as there.
+ * runs exactly bevf_msda_rows_backward (fp16 value or grad_out is an error).  grad_value must be zero-filled or
+ * hold a running sum, as there.
  *   level_hw_host  (L, 2) int32 HOST copy of level_hw (the bins are planned on the host; a device-side
  *                  mismatch is a caller bug and traps)
  *   map_range      (B, 2) int32 DEVICE: [first, end) rows of every value map (bevf_sca_plan_build)
@@ -279,7 +284,7 @@ BEVF_API int bevf_msda_dense_plan(const int32_t *level_hw_host, int L, int max_p
  * before they reach L2 (fewer reductions, more instructions; kept for A/B measurements).
  * 2: hybrid -- the coarse half of the pyramid through the splat kernel on a library-owned second stream
  * (forked from / joined to the caller's stream with events: capturable), the rest in the one kernel.
- * Results agree up to fp32 summation order.
+ * Results agree up to fp32 summation order.  Modes 1 and 2 take fp32 / bf16 only: an fp16 backward under them fails.
  */
 BEVF_API int bevf_msda_set_backward_mode(int mode);
 
@@ -359,7 +364,8 @@ BEVF_API int bevf_tsa_prep_backward(const float *raw, const float *grad_loc, con
  * preceding "self.dropout(output) + identity" of the attention / FFN
  * (temporal_self_attention.py:272, spatial_cross_attention.py:175, mmcv FFN) and TSA's
  * `query + query_pos` (temporal_self_attention.py:186-187).
- *   x, residual, pos, y, y_plus_pos: (rows, C) in `dtype`; gamma, beta: (C) in `param_dtype`;
+ *   x, residual, pos, y, y_plus_pos: (rows, C) in `dtype` (f32 | bf16 | f16); gamma, beta: (C) in `param_dtype`
+ *   (f32, or the 16-bit `dtype` itself);
  *   mean, rstd: (rows) f32.  residual / pos / y_plus_pos / mean / rstd may be NULL.  C in {256, 512}.
  *   drop_p in [0,1): inverted dropout on x with keep-mask bits from Philox4x32-10(seed, row*32+lane);
  *   the backward regenerates the same bits from `seed`, no mask tensor exists.  drop_p = 0: no dropout.
@@ -474,8 +480,8 @@ BEVF_API int bevf_linear_wgrad(const void *dy, const void *x, float *dw, float *
                                int K, void *stream);
 
 /* out[c] += sum over rows of x[r, c]  (fp32, ACCUMULATED INTO).  The bias gradient of the projections:
- * replaces the at::reduce_kernel autograd launches for nn.Linear.bias.grad.  x (rows, C) f32 | bf16. */
-/* out = srcs[0] + ... + srcs[n-1] (n <= 8 device tensors of `numel` elements, bf16 or f32, fp32 accumulation):
+ * replaces the at::reduce_kernel autograd launches for nn.Linear.bias.grad.  x (rows, C) f32 | bf16 | f16. */
+/* out = srcs[0] + ... + srcs[n-1] (n <= 8 device tensors of `numel` elements, f32, bf16 or f16, fp32 accumulation):
  * the one-pass sum of the per-layer input gradients of a shared input (replaces autograd's chain of
  * pairwise add kernels).  `srcs` is a HOST array of device pointers. */
 BEVF_API int bevf_sum_tensors(const void *const *srcs, int n, void *out, int64_t numel, int dtype, void *stream);
@@ -518,6 +524,28 @@ BEVF_API int bevf_linear_wgrad_out(const void *dy, const void *x, void *dw, void
  * GPU model; the workspace is bevf_linear_wgrad_workspace_bytes(M, N, K). */
 BEVF_API int bevf_linear_wgrad_into(const void *dy, const void *x, float *dw, float *db, void *workspace,
                                     int64_t workspace_bytes, int64_t M, int N, int K, void *stream);
+
+/*
+ * The projections above with the operand type as an argument: `dtype` = BEVF_DTYPE_BF16 or BEVF_DTYPE_F16 for x, w,
+ * dy, the residual / addend and 16-bit outputs (wgmma .f16 / .bf16 with fp32 accumulation; the kernels and their
+ * speed are the same for both).  bias_dtype is f32 or `dtype`, y_dtype f32 or `dtype`, grad_dtype (wgrad_out) f32,
+ * bf16 or f16.  The names without _dt are these with dtype = BEVF_DTYPE_BF16.
+ */
+BEVF_API int bevf_linear_forward_dt(const void *x, const void *w, const void *bias, int bias_dtype,
+                                    const void *residual, void *y, int y_dtype, int64_t M, int N, int K,
+                                    int relu, int dtype, void *stream);
+BEVF_API int bevf_linear_dgrad_dt(const void *dy, const void *w, void *dx, int64_t M, int N, int K, int dtype,
+                                  void *stream);
+BEVF_API int bevf_linear_dgrad_acc_dt(const void *dy, const void *w, const void *addend, void *dx, int64_t M,
+                                      int N, int K, int dtype, void *stream);
+BEVF_API int bevf_linear_wgrad_dt(const void *dy, const void *x, float *dw, float *db, int64_t M, int N,
+                                  int K, int dtype, void *stream);
+BEVF_API int bevf_linear_wgrad_out_dt(const void *dy, const void *x, void *dw, void *db, int grad_dtype,
+                                      void *workspace, int64_t workspace_bytes, int64_t M, int N, int K,
+                                      int dtype, void *stream);
+BEVF_API int bevf_linear_wgrad_into_dt(const void *dy, const void *x, float *dw, float *db, void *workspace,
+                                       int64_t workspace_bytes, int64_t M, int N, int K, int dtype,
+                                       void *stream);
 
 #ifdef __cplusplus
 }
