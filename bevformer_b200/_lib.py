@@ -42,6 +42,9 @@ SIGNATURES = {
     "bevf_msda_rows_backward_mixed": (c_int, [c_void_p, c_int, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p,
                                               c_int, c_void_p, c_void_p, c_void_p, c_int, c_void_p, c_void_p, c_void_p,
                                               c_void_p] + [c_int] * 7 + [c_void_p]),
+    "bevf_msda_rows_backward_mixed_dense": (c_int, [c_void_p, c_int, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p,
+                                                    c_void_p, c_int, c_void_p, c_void_p, c_void_p, c_int, c_int,
+                                                    c_void_p, c_void_p, c_void_p, c_void_p] + [c_int] * 7 + [c_void_p]),
     "bevf_gv_merge": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_void_p]),
     "bevf_msda_fx_frac_bits": (c_int, [c_int64, c_int, c_int]),
     "bevf_msda_backward_fx": (c_int, [c_void_p, c_int, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int,

@@ -26,6 +26,7 @@
 
 #include <cstdlib>
 #include <cstring>
+#include <mutex>
 #include <type_traits>
 
 #include "msda_common.cuh"
@@ -592,7 +593,8 @@ static unsigned splat_direct_mask() {
 int dense_coarse_backward(const char *who, const int64_t *hw_dev, const int64_t *ls_dev, const int32_t *hw_host,
                           const float *loc, const float *attn, const void *grad_out, float *grad_value,
                           const int32_t *map_range, int NB, int S, int M, int L, int P, cudaStream_t st,
-                          unsigned *handled, HostLevels *host_levels);                 // msda_dense.cu
+                          unsigned *handled, HostLevels *host_levels, int first_level, unsigned need_mask,
+                          int gv_S, int gv_base);                                      // msda_dense.cu
 
 // second stream + events for the hybrid backward (created by bevf_msda_set_backward_mode(2), i.e. outside any
 // stream capture; the fork / join below is capturable)
@@ -704,8 +706,8 @@ static int launch_bwd(const char *who, const void *value, const int64_t *hw, con
             const long long per_block = (long long)(kThreads / 32) * G * iters;
             const unsigned grid = (unsigned)((rows + per_block - 1) / per_block);
             msda_bwd_d32<T, TG, true><<<grid, kThreads, 0, st>>>((const T *)value, hw, ls, loc, attn, (const TG *)go, gv, gl, ga,
-                                                               row_map, S, M, Q, L, P, (65536 + P - 1) / P, iters, rows, 0u,
-                                                               hl, mixed->amax, mixed->gv16, mixed->mask, mixed->side_start,
+                                                               row_map, S, M, Q, L, P, (65536 + P - 1) / P, iters, rows,
+                                                               done_levels, hl, mixed->amax, mixed->gv16, mixed->mask, mixed->side_start,
                                                                mixed->S_side);
             return check_launch(who);
         } else {
@@ -868,38 +870,53 @@ extern "C" int bevf_msda_rows_backward(const void *value, int value_dtype, const
 // (grad_loc, grad_attn, grad_value of the fine levels) through the one-kernel backward with those levels masked.
 // mode 1: both on the caller's stream; mode 2: the dense kernel on the library's second stream (fork / join
 // with events, capturable) -- it works out of shared memory and registers while the other is bound by L2 reductions.
-static std::atomic<int> g_dense_mode{-1};
-static int dense_mode() {
+// Setting -1 = the library default: kDenseDefault for the mixed-accumulation backward (its coarse levels have
+// hundreds of contributions per pixel, see bevf_msda_rows_backward_mixed_dense), off for
+// bevf_msda_rows_backward_dense (fp32 reductions on every other level; opt-in).
+constexpr int kDenseDefault = 2;
+static std::atomic<int> g_dense_mode{-2};                   // -2: not read from the environment yet
+static int dense_setting() {
     int v = g_dense_mode.load(std::memory_order_relaxed);
-    if (v < 0) {
+    if (v == -2) {
         const char *e = getenv("BEVF_MSDA_DENSE");
-        v = e ? atoi(e) : 0;                            // default: off until the caller (or the environment) opts in
-        if (v < 0 || v > 1) v = 1;                      // (mode 2 needs its stream: only through the setter)
+        v = -1;
+        if (e && e[0]) {
+            v = atoi(e);
+            if (v < 0 || v > 1) v = 1;                  // (mode 2 needs its stream: only through the setter)
+        }
         g_dense_mode.store(v, std::memory_order_relaxed);
     }
     return v;
 }
+static int mixed_dense_mode() {
+    const int v = dense_setting();
+    return v < 0 ? kDenseDefault : v;
+}
 static int ensure_side_stream(const char *who) {
+    static std::mutex mu;
+    std::lock_guard<std::mutex> lock(mu);
     if (g_side_stream) return 0;
-    if (cudaStreamCreateWithFlags(&g_side_stream, cudaStreamNonBlocking) != cudaSuccess) {
+    cudaStream_t s = nullptr;
+    if (cudaStreamCreateWithFlags(&s, cudaStreamNonBlocking) != cudaSuccess) {
         cudaGetLastError();
-        g_side_stream = nullptr;
         return fail("%s: cannot create the second stream", who);
     }
     for (int i = 0; i < kSideEvents; ++i) cudaEventCreateWithFlags(&g_side_events[i], cudaEventDisableTiming);
+    g_side_stream = s;
     return 0;
 }
 
 extern "C" int bevf_msda_set_dense_backward(int mode) {
-    if (mode < 0 || mode > 2)
-        return fail("%s: mode must be 0 (off), 1 (same stream) or 2 (second stream)", "bevf_msda_set_dense_backward");
+    if (mode < -1 || mode > 2)
+        return fail("%s: mode must be -1 (library default), 0 (off), 1 (same stream) or 2 (second stream)",
+                    "bevf_msda_set_dense_backward");
     if (mode == 2)
         if (int e = ensure_side_stream("bevf_msda_set_dense_backward")) return e;
     g_dense_mode.store(mode, std::memory_order_relaxed);
     return 0;
 }
 
-extern "C" int bevf_msda_get_dense_backward(void) { return dense_mode(); }
+extern "C" int bevf_msda_get_dense_backward(void) { return mixed_dense_mode(); }
 
 extern "C" int bevf_msda_rows_backward_dense(const void *value, int value_dtype, const int64_t *level_hw,
                                              const int64_t *level_start, const int32_t *level_hw_host,
@@ -917,7 +934,7 @@ extern "C" int bevf_msda_rows_backward_dense(const void *value, int value_dtype,
     unsigned handled = 0;
     HostLevels hl;
     memset(&hl, 0, sizeof(hl));
-    const int mode = dense_mode();
+    const int mode = dense_setting() < 0 ? 0 : dense_setting();
     cudaEvent_t join = nullptr;
     if (value_dtype == BEVF_DTYPE_F16 || grad_out_dtype == BEVF_DTYPE_F16)
         return fail("%s: fp32 or bf16 only (fp16 runs on bevf_msda_rows_backward)", who);
@@ -932,7 +949,7 @@ extern "C" int bevf_msda_rows_backward_dense(const void *value, int value_dtype,
             ds = g_side_stream;
         }
         const int e = dense_coarse_backward(who, level_hw, level_start, level_hw_host, loc, attn, grad_out, grad_value,
-                                            map_range, B, S, M, L, P, ds, &handled, &hl);
+                                            map_range, B, S, M, L, P, ds, &handled, &hl, 0, 0u, S, 0);
         if (join) cudaEventRecord(join, g_side_stream);
         if (e) {
             if (join) cudaStreamWaitEvent(st, join, 0);
@@ -962,19 +979,20 @@ extern "C" int bevf_msda_rows_backward_f16acc(const void *value, int value_dtype
                               M, D, R, L, P, stream, 0u, nullptr, true, &mx);
 }
 
-extern "C" int bevf_msda_rows_backward_mixed(const void *value, int value_dtype, const int64_t *level_hw,
-                                             const int64_t *level_start, const int32_t *level_hw_host,
-                                             const float *loc, const float *attn, const void *grad_out,
-                                             int grad_out_dtype, void *grad_value_fine_f16, float *grad_value_side,
-                                             const uint32_t *amax_bits, int num_f16_levels, float *grad_loc,
-                                             float *grad_attn, const int32_t *row_map, const int32_t *group_order,
-                                             int B, int S, int M, int D, int R, int L, int P, void *stream) {
-    const char *who = "bevf_msda_rows_backward_mixed";
+static int rows_backward_mixed_impl(const char *who, const void *value, int value_dtype, const int64_t *level_hw,
+                                    const int64_t *level_start, const int32_t *level_hw_host, const float *loc,
+                                    const float *attn, const void *grad_out, int grad_out_dtype,
+                                    void *grad_value_fine_f16, float *grad_value_side, const uint32_t *amax_bits,
+                                    int num_f16_levels, int first_dense_level, float *grad_loc, float *grad_attn,
+                                    const int32_t *row_map, const int32_t *group_order, const int32_t *map_range,
+                                    int B, int S, int M, int D, int R, int L, int P, void *stream) {
     if (!row_map && R > 0) return fail("%s: row_map is null", who);
     if (!level_hw_host || !grad_value_fine_f16 || !grad_value_side || !amax_bits)
         return fail("%s: null pointer argument", who);
     if (L <= 1 || L > kMaxLevels || num_f16_levels < 1 || num_f16_levels >= L)
         return fail("%s: num_f16_levels must be in [1, L - 1]", who);
+    if (map_range && (first_dense_level < num_f16_levels || first_dense_level >= L))
+        return fail("%s: first_dense_level must be in [num_f16_levels, L - 1]", who);
     if (value_dtype != BEVF_DTYPE_BF16 || D != 32) return fail("%s: needs a bf16 value tensor and head_dim 32", who);
     if (!aligned16(grad_value_fine_f16) || !aligned16(grad_value_side))
         return fail("%s: device pointers must be 16-byte aligned", who);
@@ -994,9 +1012,74 @@ extern "C" int bevf_msda_rows_backward_mixed(const void *value, int value_dtype,
     mx.mask = (1u << num_f16_levels) - 1u;
     mx.side_start = hl.start[num_f16_levels];
     mx.S_side = S - mx.side_start;
-    return msda_backward_impl(who, value, value_dtype, level_hw, level_start, loc, attn, grad_out, grad_out_dtype,
-                              grad_value_side, grad_loc, grad_attn, row_map, group_order, B, S, M, D, R, L, P, stream, 0u,
-                              &hl, false, &mx);
+    cudaStream_t st = (cudaStream_t)stream;
+    unsigned dense_levels = 0;                       // levels whose grad_value the dense kernel produced
+    cudaEvent_t join = nullptr;
+    const int mode = map_range ? mixed_dense_mode() : 0;
+    if (mode != 0 && R > 0 && grad_out_dtype == BEVF_DTYPE_BF16 && aligned16(loc) && aligned16(attn) &&
+        aligned16(grad_out)) {
+        cudaStream_t ds = st;
+        if (mode == 2 && !g_side_stream) {
+            // the library default creates its stream lazily, never inside a stream capture (a captured call without
+            // the stream runs both kernels on the caller's stream)
+            cudaStreamCaptureStatus cs = cudaStreamCaptureStatusActive;
+            if (cudaStreamIsCapturing(st, &cs) != cudaSuccess) cudaGetLastError();
+            else if (cs == cudaStreamCaptureStatusNone && ensure_side_stream(who) != 0) cudaGetLastError();
+        }
+        if (mode == 2 && g_side_stream) {
+            cudaEvent_t fork = g_side_events[g_side_ev_next.fetch_add(1) % kSideEvents];
+            join = g_side_events[g_side_ev_next.fetch_add(1) % kSideEvents];
+            cudaEventRecord(fork, st);
+            cudaStreamWaitEvent(g_side_stream, fork, 0);
+            ds = g_side_stream;
+        }
+        // the dense kernel takes exactly the levels [first_dense_level, L) or nothing: a level that it cannot take
+        // leaves them all to the reduction path (no level is split between the two)
+        const unsigned suffix = ((1u << L) - 1u) & ~((1u << first_dense_level) - 1u);
+        HostLevels dhl;
+        const int e = dense_coarse_backward(who, level_hw, level_start, level_hw_host, loc, attn, grad_out,
+                                            grad_value_side, map_range, B, S, M, L, P, ds, &dense_levels, &dhl,
+                                            first_dense_level, suffix, mx.S_side, mx.side_start);
+        if (join) cudaEventRecord(join, g_side_stream);
+        if (e) {
+            if (join) cudaStreamWaitEvent(st, join, 0);
+            return e;
+        }
+    }
+    const int e = msda_backward_impl(who, value, value_dtype, level_hw, level_start, loc, attn, grad_out, grad_out_dtype,
+                                     grad_value_side, grad_loc, grad_attn, row_map, group_order, B, S, M, D, R, L, P,
+                                     stream, dense_levels, &hl, false, &mx);
+    if (join) cudaStreamWaitEvent(st, join, 0);
+    return e;
+}
+
+extern "C" int bevf_msda_rows_backward_mixed(const void *value, int value_dtype, const int64_t *level_hw,
+                                             const int64_t *level_start, const int32_t *level_hw_host,
+                                             const float *loc, const float *attn, const void *grad_out,
+                                             int grad_out_dtype, void *grad_value_fine_f16, float *grad_value_side,
+                                             const uint32_t *amax_bits, int num_f16_levels, float *grad_loc,
+                                             float *grad_attn, const int32_t *row_map, const int32_t *group_order,
+                                             int B, int S, int M, int D, int R, int L, int P, void *stream) {
+    return rows_backward_mixed_impl("bevf_msda_rows_backward_mixed", value, value_dtype, level_hw, level_start,
+                                    level_hw_host, loc, attn, grad_out, grad_out_dtype, grad_value_fine_f16,
+                                    grad_value_side, amax_bits, num_f16_levels, L, grad_loc, grad_attn, row_map,
+                                    group_order, nullptr, B, S, M, D, R, L, P, stream);
+}
+
+extern "C" int bevf_msda_rows_backward_mixed_dense(const void *value, int value_dtype, const int64_t *level_hw,
+                                                   const int64_t *level_start, const int32_t *level_hw_host,
+                                                   const float *loc, const float *attn, const void *grad_out,
+                                                   int grad_out_dtype, void *grad_value_fine_f16,
+                                                   float *grad_value_side, const uint32_t *amax_bits,
+                                                   int num_f16_levels, int first_dense_level, float *grad_loc,
+                                                   float *grad_attn, const int32_t *row_map, const int32_t *map_range,
+                                                   int B, int S, int M, int D, int R, int L, int P, void *stream) {
+    const char *who = "bevf_msda_rows_backward_mixed_dense";
+    if (!map_range) return fail("%s: null pointer argument", who);
+    return rows_backward_mixed_impl(who, value, value_dtype, level_hw, level_start, level_hw_host, loc, attn, grad_out,
+                                    grad_out_dtype, grad_value_fine_f16, grad_value_side, amax_bits, num_f16_levels,
+                                    first_dense_level, grad_loc, grad_attn, row_map, nullptr, map_range, B, S, M, D, R,
+                                    L, P, stream);
 }
 
 namespace bevf {

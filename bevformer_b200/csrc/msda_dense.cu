@@ -154,13 +154,15 @@ __device__ __forceinline__ unsigned short bf16_add(unsigned short old, float x) 
 //            fence.proxy.async -> arrive full[t]
 //   issuers: wait full[t] -> wgmma for every touched 64-pixel half of their tiles -> wgmma.wait_group -> empty[t]
 // so the scatter of up to NT - 1 further steps runs under the MMAs of the previous ones.
+// grad_value is (NB, gv_S, M, 32) and holds the pixels [gv_base, gv_base + gv_S) of every map: the whole pyramid
+// (gv_S = S, gv_base = 0), or the fp32 side buffer of the mixed accumulation (gv_base = its first pixel).
 template <int kTiles, int P, int NT>
 __global__ void __launch_bounds__(128 * NT + 256, 1)
 msda_bwd_dense_tc(const __grid_constant__ DenseBins bins, const int64_t *__restrict__ level_hw,
                   const int64_t *__restrict__ level_start, const float *__restrict__ loc,
                   const float *__restrict__ attn, const bf16 *__restrict__ grad_out,
-                  float *__restrict__ grad_value, const int *__restrict__ map_range, int NB, int S, int M, int L,
-                  int chunk_rows, int dbg) {
+                  float *__restrict__ grad_value, const int *__restrict__ map_range, int NB, int gv_S, int gv_base,
+                  int M, int L, int chunk_rows, int dbg) {
     static_assert(P == 4 || P == 8, "points per level: 4 or 8");
     static_assert(kTiles == 4, "accumulator tiles per bin: 2 per issuer warpgroup");
     static_assert(NT >= 1 && NT <= 3, "scatter teams");
@@ -469,7 +471,7 @@ msda_bwd_dense_tc(const __grid_constant__ DenseBins bins, const int64_t *__restr
                             const bool nz = ((__float_as_uint(v.x) | __float_as_uint(v.y) | __float_as_uint(v.z) |
                                               __float_as_uint(v.w)) & 0x7fffffffu) != 0u;
                             if (nz && row < nb) {
-                                float *gp = grad_value + (((long long)b * S + s0 + row) * M + m) * 32 + sub * 4;
+                                float *gp = grad_value + (((long long)b * gv_S + s0 - gv_base + row) * M + m) * 32 + sub * 4;
                                 red_add_v4(gp, v.x, v.y, v.z, v.w);
                             }
                         }
@@ -494,10 +496,12 @@ static long dense_env(const char *name, long dflt) {
     return e ? strtol(e, nullptr, 0) : dflt;
 }
 
-// Bins of at most `cap` consecutive pixels over the levels with at most `max_pix` pixels: a level larger than a bin
-// is cut into ceil(n / cap) bins, consecutive small levels share one (the kernel gives each level of a bin its own
-// group of scatter threads).  Returns the mask of the covered levels, -1 for a bad shape, -2 if the table overflows.
-static int plan_dense_bins(const int32_t *hw_host, int L, long max_pix, int cap, DenseBins &bins, long long *total) {
+// Bins of at most `cap` consecutive pixels over the levels l >= first with at most `max_pix` pixels: a level larger
+// than a bin is cut into ceil(n / cap) bins, consecutive small levels share one (the kernel gives each level of a bin
+// its own group of scatter threads).  Returns the mask of the covered levels, -1 for a bad shape, -2 if the table
+// overflows.
+static int plan_dense_bins(const int32_t *hw_host, int L, long max_pix, int cap, DenseBins &bins, long long *total,
+                           int first = 0) {
     memset(&bins, 0, sizeof(bins));
     bins.L = L;
     long long start = 0;
@@ -508,7 +512,7 @@ static int plan_dense_bins(const int32_t *hw_host, int L, long max_pix, int cap,
         if (h <= 0 || w <= 0 || h >= 32768 || w >= 32768) return -1;
         const long long n = (long long)h * w;
         bins.hl.h[l] = h; bins.hl.w[l] = w; bins.hl.start[l] = (int)start;
-        if (n <= max_pix) {
+        if (l >= first && n <= max_pix) {
             if (n <= cap && open >= 0 && bins.n[open] + n <= cap && bins.nlev[open] < kDnBinLevels) {
                 bins.lev[open][bins.nlev[open]++] = l;   // contiguous with the previous coarse level
                 bins.n[open] += (int)n;
@@ -536,13 +540,16 @@ static int plan_dense_bins(const int32_t *hw_host, int L, long max_pix, int cap,
     return (int)mask;
 }
 
-// Plans the bins from the HOST copy of the pyramid and launches the dense kernel for every level with at most
-// `BEVF_DENSE_MAXPIX` pixels.  *handled = mask of the levels whose grad_value it produced (0: not applicable --
-// the caller then leaves every level to the reduction path).
+// Plans the bins from the HOST copy of the pyramid and launches the dense kernel for every level l >= first_level
+// with at most `BEVF_DENSE_MAXPIX` pixels.  *handled = mask of the levels whose grad_value it produced (0: not
+// applicable -- the caller then leaves every level to the reduction path).  need_mask != 0: launch only if the
+// covered levels are exactly those (the mixed accumulation hands the dense kernel a whole suffix of the pyramid).
+// grad_value, gv_S, gv_base: see msda_bwd_dense_tc.
 int dense_coarse_backward(const char *who, const int64_t *hw_dev, const int64_t *ls_dev, const int32_t *hw_host,
                           const float *loc, const float *attn, const void *grad_out, float *grad_value,
                           const int32_t *map_range, int NB, int S, int M, int L, int P, cudaStream_t st,
-                          unsigned *handled, HostLevels *host_levels) {
+                          unsigned *handled, HostLevels *host_levels, int first_level, unsigned need_mask,
+                          int gv_S, int gv_base) {
     *handled = 0;
     static const long max_pix = dense_env("BEVF_DENSE_MAXPIX", 8192);
     static const long tiles = dense_env("BEVF_DENSE_TILES", 4);
@@ -553,12 +560,12 @@ int dense_coarse_backward(const char *who, const int64_t *hw_dev, const int64_t 
     const int cap = (int)tiles * 128;
     DenseBins bins;
     long long start = 0;
-    const int pm = plan_dense_bins(hw_host, L, max_pix, cap, bins, &start);
+    const int pm = plan_dense_bins(hw_host, L, max_pix, cap, bins, &start, first_level);
     if (pm == -1) return fail("%s: bad host level shape", who);
     if (pm == -2) return 0;                              // pyramid too large for the bin table
     const unsigned mask = (unsigned)pm;
     if (start != S) return fail("%s: host level shapes do not add up to S (%lld vs %lld)", who, start, S);
-    if (mask == 0) return 0;
+    if (mask == 0 || (need_mask != 0 && mask != need_mask)) return 0;
     static int sms = 0;
     if (sms == 0) {
         int dev = 0;
@@ -566,7 +573,7 @@ int dense_coarse_backward(const char *who, const int64_t *hw_dev, const int64_t 
         cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
     }
     static const long teams_env = dense_env("BEVF_DENSE_TEAMS", 0);
-    const int teams = teams_env > 0 ? (int)teams_env : 2;
+    const int teams = teams_env > 0 ? (int)teams_env : 3;     // 3: 12-15 % faster than 2 on the base SCA launch (H100)
     const size_t smem = 1024 + (size_t)teams * ((size_t)tiles * kDnTileBytes + 4096) + 8 * kDnTransposeBytes + 256;
     static const long dbg = dense_env("BEVF_DENSE_DEBUG", 0);       // development: 1 = no MMAs, 2 = no scatter, 4 = no flush, 8 = every tile counts as touched
     auto launch = [&](auto kern) -> int {
@@ -587,7 +594,8 @@ int dense_coarse_backward(const char *who, const int64_t *hw_dev, const int64_t 
             }
         }
         kern<<<(unsigned)sms, 128 * teams + 256, smem, st>>>(bins, hw_dev, ls_dev, loc, attn, (const bf16 *)grad_out,
-                                                           grad_value, map_range, NB, S, M, L, (int)chunk, (int)dbg);
+                                                           grad_value, map_range, NB, gv_S, gv_base, M, L, (int)chunk,
+                                                           (int)dbg);
         return check_launch(who);
     };
     int e;

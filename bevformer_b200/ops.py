@@ -363,6 +363,23 @@ def gv_mode_for(rows_per_map: float, num_points: int, level_hw_host):
     return "f16" if nfine == len(shapes) else ("mixed", shapes, nfine)
 
 
+def dense_levels_for(rows_per_map: float, num_points: int, level_hw_host):
+    """First level of the suffix of the pyramid whose grad_value the mixed backward hands to the dense tensor-core
+    kernel (bevf_msda_rows_backward_mixed_dense), or None: the levels on which a (pixel, head) collects on average
+    more than 256 contributions (rows_per_map * num_points * 4 / (H * W), as in gv_mode_for).  Every level costs the
+    reduction path the same number of sectors, but the dense kernel's cost grows with the pixels of its levels.
+    Measured on the base SCA launch (H100 SXM, 400 W; tools/bench_sca_backward.py): level 3 alone (630 per pixel)
+    1.48 ms against 1.67 ms for the fp32 reductions, levels 2-3 (from 164) 1.74 ms, levels 1-3 (from 41) 3.07 ms."""
+    shapes = [(int(h), int(w)) for h, w in level_hw_host]
+    first = None
+    for l in range(len(shapes) - 1, -1, -1):
+        h, w = shapes[l]
+        if rows_per_map * num_points * 4.0 / (h * w) <= 256:
+            break
+        first = l
+    return first
+
+
 class LazyGradValue:
     """grad_value of a sampler backward still in accumulator form (scaled fp16 [+ fp32 side buffer]): ``materialize()``
     runs the one conversion pass (bevf_gv16_unscale / bevf_gv_merge) on the CURRENT stream and returns the bf16
@@ -505,10 +522,14 @@ def msda_rows_backward_f16acc(value, spatial_shapes, level_start_index, loc, att
 
 
 def msda_rows_backward_mixed(value, spatial_shapes, level_start_index, level_hw_host, num_f16_levels, loc, attn,
-                             row_map, grad_output, group_order=None, lazy=False):
+                             row_map, grad_output, group_order=None, lazy=False, map_range=None,
+                             first_dense_level=None):
     """Row-list backward with MIXED accumulation (bevf_msda_rows_backward_mixed): the first ``num_f16_levels`` levels
     in scaled fp16, the others in fp32 into a side buffer that only spans their pixels; one merge pass produces the
-    bf16 gradient.  ``level_hw_host``: [(h, w), ...] python ints that MUST equal the device spatial_shapes."""
+    bf16 gradient.  ``level_hw_host``: [(h, w), ...] python ints that MUST equal the device spatial_shapes.
+    ``map_range`` (B, 2) int32 for row lists grouped by value map (instead of ``group_order``): the levels
+    [first_dense_level, L) (default: every side level) come from the dense tensor-core kernel where its plan covers
+    them (bevf_msda_rows_backward_mixed_dense)."""
     import ctypes
     for t, n in ((value, "value"), (loc, "sampling_loc"), (attn, "attn_weight"), (row_map, "row_map"),
                  (grad_output, "grad_output")):
@@ -520,6 +541,10 @@ def msda_rows_backward_mixed(value, spatial_shapes, level_start_index, level_hw_
     R, _, L, P, _ = loc.shape
     if len(level_hw_host) != L or not (1 <= num_f16_levels < L):
         raise RuntimeError("mixed-accumulation backward: level_hw_host / num_f16_levels do not fit the pyramid")
+    if map_range is not None:
+        _need_cuda(map_range, "map_range")
+        if group_order is not None or map_range.numel() != 2 * NB or map_range.dtype != torch.int32:
+            raise RuntimeError("mixed-accumulation backward: map_range must be (B, 2) int32, without group_order")
     ss, ls = _level_tensors(value, spatial_shapes, level_start_index)
     s_fine = sum(int(h) * int(w) for h, w in level_hw_host[:num_f16_levels])
     grad_output = grad_output.contiguous()
@@ -531,12 +556,17 @@ def msda_rows_backward_mixed(value, spatial_shapes, level_start_index, level_hw_
         amax = abs_max_bits(grad_output)
         fine = torch.zeros((NB, s_fine, M, D), device=value.device, dtype=torch.float16)
         side = torch.zeros((NB, S - s_fine, M, D), device=value.device, dtype=torch.float32)
-        st = lib.bevf_msda_rows_backward_mixed(value.data_ptr(), _DT[value.dtype], ss.data_ptr(), ls.data_ptr(),
-                                               ctypes.addressof(hw), loc.data_ptr(), attn.data_ptr(),
-                                               grad_output.data_ptr(), _DT[grad_output.dtype], fine.data_ptr(),
-                                               side.data_ptr(), amax.data_ptr(), int(num_f16_levels),
-                                               grad_loc.data_ptr(), grad_attn.data_ptr(), row_map.data_ptr(),
-                                               _ptr(group_order), NB, S, M, D, R, L, P, _stream_ptr(value))
+        args = (value.data_ptr(), _DT[value.dtype], ss.data_ptr(), ls.data_ptr(), ctypes.addressof(hw), loc.data_ptr(),
+                attn.data_ptr(), grad_output.data_ptr(), _DT[grad_output.dtype], fine.data_ptr(), side.data_ptr(),
+                amax.data_ptr(), int(num_f16_levels))
+        tail = (grad_loc.data_ptr(), grad_attn.data_ptr(), row_map.data_ptr())
+        if map_range is None:
+            st = lib.bevf_msda_rows_backward_mixed(*args, *tail, _ptr(group_order), NB, S, M, D, R, L, P,
+                                                   _stream_ptr(value))
+        else:
+            kd = num_f16_levels if first_dense_level is None else int(first_dense_level)
+            st = lib.bevf_msda_rows_backward_mixed_dense(*args, kd, *tail, map_range.data_ptr(), NB, S, M, D, R, L, P,
+                                                         _stream_ptr(value))
         _lib.check(st, lib)
     gv = LazyGradValue(value.shape, fine, side, amax)
     return (gv if lazy else gv.materialize()), grad_loc, grad_attn
@@ -609,8 +639,7 @@ class SamplerRows(Function):
         if ctx.gv_zero is not None:
             gv0, done = ctx.gv_zero
             torch.cuda.current_stream(value.device).wait_event(done)
-        dense_on = ctx.dense is not None and _lib.load().bevf_msda_get_dense_backward() != 0   # explicit opt-in wins
-        if ctx.gv_mode is not None and gv0 is None and grad_out.dtype == torch.bfloat16 and not dense_on:
+        if ctx.gv_mode is not None and gv0 is None and grad_out.dtype == torch.bfloat16:
             if ctx.gv_mode == "f16":
                 gv, gl, ga = msda_rows_backward_f16acc(value, ss, ls, loc, attn, row_map, grad_out, ctx.group_order,
                                                        lazy=True)
@@ -623,11 +652,22 @@ class SamplerRows(Function):
                     if ctx.value_early is not None and ctx.value_early(gv):
                         return None, gl, ga, None, None, None, None, None, None
                     return gv.to(value.dtype), gl, ga, None, None, None, None, None, None
-                gv, gl, ga = msda_rows_backward_mixed(value, ss, ls, hw_host, nfine, loc, attn, row_map, grad_out,
-                                                      ctx.group_order, lazy=True)
+                kd = None
+                if ctx.dense is not None and ctx.group_order is None and _lib.load().bevf_msda_get_dense_backward():
+                    kd = dense_levels_for(row_map.numel() / max(1, value.shape[0]), loc.shape[3], hw_host)
+                if kd is not None:
+                    # levels [nfine, kd) fp32 reductions, [kd, L) on the tensor cores, both into the side buffer
+                    gv, gl, ga = msda_rows_backward_mixed(value, ss, ls, hw_host, nfine, loc, attn, row_map, grad_out,
+                                                          lazy=True, map_range=ctx.dense[1],
+                                                          first_dense_level=max(kd, nfine))
+                else:
+                    gv, gl, ga = msda_rows_backward_mixed(value, ss, ls, hw_host, nfine, loc, attn, row_map, grad_out,
+                                                          ctx.group_order, lazy=True)
             if ctx.value_early is not None and ctx.value_early(gv):
                 return None, gl, ga, None, None, None, None, None, None      # the producer converts it off the critical path
             return gv.materialize(), gl, ga, None, None, None, None, None, None
+        # (the coarse levels of an fp32-accumulated pyramid go to the dense kernel only where the caller opted in:
+        # bevf_msda_rows_backward_dense is off under the library default)
         gv, gl, ga = msda_rows_backward(value, ss, ls, loc, attn, row_map, grad_out.contiguous(), gv0,
                                         group_order=ctx.group_order, dense=ctx.dense)
         if ctx.value_early is not None and ctx.value_early(gv):

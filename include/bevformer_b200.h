@@ -162,6 +162,17 @@ BEVF_API int bevf_msda_rows_backward_ordered(const void *value, int value_dtype,
  *                                             taken from level_hw_host (L, 2) int32 HOST, the kernel re-derives which
  *                                             levels lie before / after it from the DEVICE pyramid (a device level
  *                                             that straddles S_fine is a caller bug and traps)
+ *   bevf_msda_rows_backward_mixed_dense       bevf_msda_rows_backward_mixed for row lists grouped by value map
+ *                                             (map_range (B, 2) int32 DEVICE, as bevf_msda_rows_backward_dense; no
+ *                                             group_order): the side levels [first_dense_level, L) (first_dense_level
+ *                                             in [num_f16_levels, L - 1]) come from the dense tensor-core kernel
+ *                                             (csrc/msda_dense.cu) instead of fp32 L2 reductions, written into
+ *                                             grad_value_side, on the stream bevf_msda_set_dense_backward selects.
+ *                                             Only if its bin plan covers exactly those levels, grad_out is
+ *                                             bf16 and there are 4 or 8 points per level; otherwise, with the dense
+ *                                             mode 0, or when the device pyramid differs from level_hw_host, this is
+ *                                             exactly bevf_msda_rows_backward_mixed.  Same outputs either way; the
+ *                                             dense levels' coefficients are rounded to bf16 (2^-9 relative per term).
  *   bevf_gv_merge(fine, side, amax, out, B, S, S_fine, row_elems)   out (B, S, row_elems) bf16 from both
  * All need a bf16 value tensor and head_dim 32 (fp16 value is an error); grad_loc / grad_attn are those of the fp32
  * path bit for bit.
@@ -181,6 +192,14 @@ BEVF_API int bevf_msda_rows_backward_mixed(const void *value, int value_dtype, c
                                            const uint32_t *amax_bits, int num_f16_levels, float *grad_loc,
                                            float *grad_attn, const int32_t *row_map, const int32_t *group_order,
                                            int B, int S, int M, int D, int R, int L, int P, void *stream);
+BEVF_API int bevf_msda_rows_backward_mixed_dense(const void *value, int value_dtype, const int64_t *level_hw,
+                                                 const int64_t *level_start, const int32_t *level_hw_host,
+                                                 const float *loc, const float *attn, const void *grad_out,
+                                                 int grad_out_dtype, void *grad_value_fine_f16, float *grad_value_side,
+                                                 const uint32_t *amax_bits, int num_f16_levels, int first_dense_level,
+                                                 float *grad_loc, float *grad_attn, const int32_t *row_map,
+                                                 const int32_t *map_range,
+                                                 int B, int S, int M, int D, int R, int L, int P, void *stream);
 BEVF_API int bevf_gv_merge(const void *fine_f16, const float *side_f32, const uint32_t *amax_bits, void *out_bf16,
                            int B, int S, int S_fine, int row_elems, void *stream);
 
@@ -256,9 +275,12 @@ BEVF_API int bevf_msda_rows_forward_staged(const void *value, int value_dtype, c
  *   level_hw_host  (L, 2) int32 HOST copy of level_hw (the bins are planned on the host; a device-side
  *                  mismatch is a caller bug and traps)
  *   map_range      (B, 2) int32 DEVICE: [first, end) rows of every value map (bevf_sca_plan_build)
- * bevf_msda_set_dense_backward: 0 = never use the dense kernel, 1 = on the caller's stream (default, or the
- * environment variable BEVF_MSDA_DENSE), 2 = on a library-owned second stream next to the reduction kernel
- * (fork / join with events, capturable).
+ * bevf_msda_set_dense_backward (process-wide): 0 = never use the dense kernel, 1 = on the caller's stream,
+ * 2 = on a library-owned second stream next to the reduction kernel (fork / join with events, capturable),
+ * -1 = the library default: mode 2 for bevf_msda_rows_backward_mixed_dense, off for bevf_msda_rows_backward_dense.
+ * The environment variable BEVF_MSDA_DENSE=0 / 1 replaces the default.  Under the default the second stream is
+ * created at the first call that is not being captured; a captured call before that runs on the caller's stream.
+ * bevf_msda_get_dense_backward returns the mode bevf_msda_rows_backward_mixed_dense runs in (0, 1 or 2).
  */
 BEVF_API int bevf_msda_rows_backward_dense(const void *value, int value_dtype, const int64_t *level_hw,
                                            const int64_t *level_start, const int32_t *level_hw_host,
