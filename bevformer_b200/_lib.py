@@ -65,6 +65,12 @@ SIGNATURES = {
                                               c_void_p, c_int, c_void_p] + [c_int] * 7 + [c_void_p]),
     "bevf_sca_prep_forward": (c_int, [c_void_p] * 7 + [c_int] * 8 + [c_void_p]),
     "bevf_sca_prep_backward": (c_int, [c_void_p] * 6 + [c_int] * 8 + [c_void_p]),
+    "bevf_sca_rows_forward_fused": (c_int, [c_void_p, c_int] + [c_void_p] * 9 + [c_int, c_void_p, c_int, c_void_p]
+                                    + [c_int] * 12 + [c_void_p]),
+    "bevf_sca_rows_backward_fused": (c_int, [c_void_p, c_int] + [c_void_p] * 7 + [c_int] + [c_void_p] * 5
+                                     + [c_int, c_void_p, c_void_p, c_void_p, c_int, c_int] + [c_void_p] * 5
+                                     + [c_int] * 12 + [c_void_p]),
+    "bevf_sca_prep_backward_multi": (c_int, [c_void_p] * 6 + [c_int] * 8 + [c_void_p]),
     "bevf_tsa_prep_forward": (c_int, [c_void_p] * 5 + [c_int] * 6 + [c_void_p]),
     "bevf_tsa_prep_backward": (c_int, [c_void_p] * 5 + [c_int] * 7 + [c_void_p]),
     "bevf_layernorm_forward": (c_int, [c_void_p] * 4 + [c_int] + [c_void_p] * 5

@@ -63,6 +63,17 @@ typedef __nv_bfloat16 bf16;
 // the ~10-ulp __expf).  The softmaxes of the sampling heads use it: their gradients feed sums with heavy cancellation.
 __device__ __forceinline__ float exp_rn(float x) { return (float)exp((double)x); }
 
+// max / sum over the 4 lanes of an aligned quad (every lane of the warp takes part).  The sampling-head softmaxes
+// reduce a head's partial sums with these; the SCA prep kernels and the fused sampler must use the same order.
+__device__ __forceinline__ float quad_max(float v) {
+    v = fmaxf(v, __shfl_xor_sync(0xffffffffu, v, 1));
+    return fmaxf(v, __shfl_xor_sync(0xffffffffu, v, 2));
+}
+__device__ __forceinline__ float quad_sum(float v) {
+    v += __shfl_xor_sync(0xffffffffu, v, 1);
+    return v + __shfl_xor_sync(0xffffffffu, v, 2);
+}
+
 __device__ __forceinline__ float bf16_lo(uint32_t u) { return __uint_as_float(u << 16); }
 __device__ __forceinline__ float bf16_hi(uint32_t u) { return __uint_as_float(u & 0xffff0000u); }
 

@@ -127,14 +127,6 @@ sca_prep_bwd(const float *__restrict__ raw, const float *__restrict__ grad_loc,
 // Every global access is a 16 B vector and a quad covers a head's contiguous 32*PPL/8.. bytes, so
 // the warp reads / writes whole 128 B lines; the softmax reduces over the quad with two shuffles.
 // ------------------------------------------------------------------------------------------------
-__device__ __forceinline__ float quad_max(float v) {
-    v = fmaxf(v, __shfl_xor_sync(0xffffffffu, v, 1));
-    return fmaxf(v, __shfl_xor_sync(0xffffffffu, v, 2));
-}
-__device__ __forceinline__ float quad_sum(float v) {
-    v += __shfl_xor_sync(0xffffffffu, v, 1);
-    return v + __shfl_xor_sync(0xffffffffu, v, 2);
-}
 template <int N> __device__ __forceinline__ void ldv(const float *p, float (&v)[N]) {
     if constexpr (N % 4 == 0) {
 #pragma unroll
@@ -231,7 +223,9 @@ sca_prep_fwd_m8(const float *__restrict__ raw, const float *__restrict__ ref_cam
     stv<PPL>(attn + (t * M + m) * LP + k0, lg);
 }
 
-template <int PPL, typename TO>
+// kMultiOnly: the queries seen by exactly one camera are skipped -- the fused sampler backward
+// (bevf_sca_rows_backward_fused) has finished their d_raw rows itself
+template <int PPL, typename TO, bool kMultiOnly = false>
 __global__ void __launch_bounds__(kEThreads)
 sca_prep_bwd_m8(const float *__restrict__ raw, const float *__restrict__ grad_loc,
                 const float *__restrict__ grad_attn, const int *__restrict__ pair_of,
@@ -245,6 +239,11 @@ sca_prep_bwd_m8(const float *__restrict__ raw, const float *__restrict__ grad_lo
     const long long bq = (long long)blockIdx.x * (kEThreads / 32) + (threadIdx.x >> 5);
     if (bq >= (long long)B * Nq) return;
     const int q = (int)(bq % Nq), b = (int)(bq / Nq);
+    if constexpr (kMultiOnly) {
+        int seen = 0;
+        for (int c = 0; c < ncam; ++c) seen += __ldg(pair_of + (long long)c * Nq + q) >= 0 ? 1 : 0;
+        if (seen == 1) return;                           // warp-uniform
+    }
     const int LP = 4 * PPL, k0 = sub * PPL;
     const long long rbase = bq * (M * LP * 3);
     float a[PPL];
@@ -1056,6 +1055,34 @@ extern "C" int bevf_sca_prep_backward(const float *raw, const float *grad_loc,
     if (out_dtype == BEVF_DTYPE_F16)
         return sca_prep_backward_t<__half>(who, raw, grad_loc, grad_attn, pair_of, level_hw, (__half *)d_raw, B, Nq, R, M, L, P, ncam, st);
     return sca_prep_backward_t<float>(who, raw, grad_loc, grad_attn, pair_of, level_hw, (float *)d_raw, B, Nq, R, M, L, P, ncam, st);
+}
+
+template <typename TO>
+static void sca_prep_backward_multi_t(const float *raw, const float *grad_loc, const float *grad_attn,
+                                      const int32_t *pair_of, const int64_t *level_hw, TO *d_raw, int B, int Nq,
+                                      int R, int L, int P, int ncam, cudaStream_t st) {
+    const int pmagic = (65536 + P - 1) / P;
+    const unsigned wgrid = blocks_for((long long)B * Nq, kEThreads / 32);
+    sca_prep_bwd_m8<8, TO, true><<<wgrid, kEThreads, 0, st>>>(raw, grad_loc, grad_attn, pair_of, level_hw, d_raw, B,
+                                                              Nq, R, L, P, ncam, pmagic);
+}
+
+extern "C" int bevf_sca_prep_backward_multi(const float *raw, const float *grad_loc,
+                                            const float *grad_attn, const int32_t *pair_of,
+                                            const int64_t *level_hw, void *d_raw, int out_dtype, int B, int Nq,
+                                            int R, int M, int L, int P, int ncam, void *stream) {
+    const char *who = "bevf_sca_prep_backward_multi";
+    BEVF_REQUIRE(B >= 0 && Nq >= 0 && R >= 0 && L > 0 && P > 0 && ncam > 0 && ncam <= 16, who, "bad dimension (ncam <= 16)");
+    BEVF_REQUIRE(M == 8 && L * P == 32 && L <= 16, who, "8 heads and num_levels * num_points == 32 only");
+    BEVF_REQUIRE(out_dtype == BEVF_DTYPE_BF16 || out_dtype == BEVF_DTYPE_F16, who, "bf16 or fp16 d_raw only");
+    if ((long long)B * Nq == 0) return 0;
+    BEVF_REQUIRE(raw && pair_of && level_hw && d_raw && (R == 0 || (grad_loc && grad_attn)), who, "null pointer argument");
+    cudaStream_t st = (cudaStream_t)stream;
+    if (out_dtype == BEVF_DTYPE_BF16)
+        sca_prep_backward_multi_t<bf16>(raw, grad_loc, grad_attn, pair_of, level_hw, (bf16 *)d_raw, B, Nq, R, L, P, ncam, st);
+    else
+        sca_prep_backward_multi_t<__half>(raw, grad_loc, grad_attn, pair_of, level_hw, (__half *)d_raw, B, Nq, R, L, P, ncam, st);
+    return check_launch(who);
 }
 
 extern "C" int bevf_tsa_prep_forward(const float *raw, const float *ref2d, const int64_t *level_hw,

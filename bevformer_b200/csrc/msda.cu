@@ -36,15 +36,20 @@ namespace bevf {
 // ------------------------------------------------------------------------------------------------
 // forward, head_dim == 32
 // ------------------------------------------------------------------------------------------------
-template <typename T, typename TO>
+// kFused: loc / attn are derived from SCA's raw head output (ScaFuse, msda_common.cuh).  A prologue computes the row's
+// softmax statistics (stored for the backward) and its 32 attention weights, which the produce phase reads back from
+// shared memory; the samples of the levels the dense backward takes are also stored (ScaFuse::coarse_*)
+template <typename T, typename TO, bool kFused = false>
 __global__ void __launch_bounds__(kThreads)
 msda_fwd_d32(const T *__restrict__ value, const int64_t *__restrict__ level_hw,
              const int64_t *__restrict__ level_start, const float *__restrict__ loc,
              const float *__restrict__ attn, TO *__restrict__ out,
              const int *__restrict__ row_map, int S, int M, int Q, int L, int P, int magic,
-             int iters, long long rows) {
+             int iters, long long rows, const __grid_constant__ ScaFuse fz = ScaFuse{}) {
     constexpr int VEC = Vec<T>::N, LANES = 32 / VEC, G = 32 / LANES;
+    static_assert(!kFused || LANES == 4, "the fused prep needs 4 lanes per row (16-bit value rows)");
     constexpr bool kHalf = std::is_same<T, bf16>::value;   // bf16: packed bf16 weights (fhfma); fp16: fp32 weights
+    __shared__ __align__(16) float s_fa[kFused ? kThreads / 32 * G : 1][kFuseLP];   // attn of each row group
     __shared__ LevelTab tab;
     load_level_tab(level_hw, level_start, L, M * 32, tab);
 
@@ -65,6 +70,18 @@ msda_fwd_d32(const T *__restrict__ value, const int64_t *__restrict__ level_hw,
     const T *vbase = value + ((long long)b * S * M + m) * 32 + sub * VEC;
     const float2 *locp = reinterpret_cast<const float2 *>(loc) + row * LP;
     const float *attp = attn + row * LP;
+    ScaRow sr;
+    const int fgrp = warp * G + grp;
+    if constexpr (kFused) {
+        live = live && sca_row(fz, row, sr);
+        float fa[8];
+        const float2 st = sca_row_stats(sr, live, sub, fa);
+        if (live && sub == 0) fz.stats[row] = st;
+        __syncwarp();                                 // the previous row group's reads of s_fa are done
+        *reinterpret_cast<float4 *>(&s_fa[fgrp][8 * sub]) = make_float4(fa[0], fa[1], fa[2], fa[3]);
+        *reinterpret_cast<float4 *>(&s_fa[fgrp][8 * sub + 4]) = make_float4(fa[4], fa[5], fa[6], fa[7]);
+        __syncwarp();
+    }
 
     float acc[VEC];
 #pragma unroll
@@ -78,8 +95,20 @@ msda_fwd_d32(const T *__restrict__ value, const int64_t *__restrict__ level_hw,
         bool valid = false;
         if (sm < LP && live) {
             const int l = level_of(sm, magic);
-            const float2 xy = __ldg(locp + sm);
-            const float a = __ldg(attp + sm);
+            float2 xy;
+            float a;
+            if constexpr (kFused) {
+                sca_loc(sr, sm, l, P, fz.Dz, tab.h[l], tab.w[l], xy.x, xy.y);
+                a = s_fa[fgrp][sm];
+                if (l >= fz.coarse_from) {
+                    const long long ci = row * (LP - fz.coarse_from * P) + (sm - fz.coarse_from * P);
+                    fz.coarse_loc[ci] = xy;
+                    fz.coarse_attn[ci] = a;
+                }
+            } else {
+                xy = __ldg(locp + sm);
+                a = __ldg(attp + sm);
+            }
             const Corner c = make_corner(xy.x, xy.y, tab.h[l], tab.w[l]);
             enc = (c.pidx * pix) | c.dx | (c.dy << 1);
             valid = c.valid;
@@ -132,7 +161,10 @@ msda_fwd_d32(const T *__restrict__ value, const int64_t *__restrict__ level_hw,
 // power of two that puts max|grad_out| into [8, 16), gv16_scale(*gv_amax)); meant for maps where a pixel collects
 // few contributions, e.g. TemporalSelfAttention's single fine level (bf16 accumulation was measured at 1.4e-2 of
 // max|grad_value| there -- above the 1e-2 bar; fp16 has three more mantissa bits).
-template <typename T, typename TG, bool kScatter, typename TV = float>
+// kFused: loc / attn are recomputed from SCA's raw head output and the forward's softmax statistics (ScaFuse), and
+// the row epilogue finishes d_raw (sca_prep_bwd_m8's arithmetic) for the queries that exactly one camera sees; the
+// rows of the other queries store grad_loc / grad_attn for bevf_sca_prep_backward_multi as before.
+template <typename T, typename TG, bool kScatter, typename TV = float, bool kFused = false>
 __global__ void __launch_bounds__(kThreads)
 msda_bwd_d32(const T *__restrict__ value, const int64_t *__restrict__ level_hw,
              const int64_t *__restrict__ level_start, const float *__restrict__ loc,
@@ -142,7 +174,8 @@ msda_bwd_d32(const T *__restrict__ value, const int64_t *__restrict__ level_hw,
              int L, int P, int magic, int iters, long long rows, unsigned red_skip,
              const __grid_constant__ HostLevels host_levels, const unsigned *__restrict__ gv_amax = nullptr,
              __half *__restrict__ gv16 = nullptr, unsigned gv16_mask = 0u, int side_start = 0, int S_side = 0,
-             const unsigned *__restrict__ fx_bounds = nullptr, int fx_bits = 0) {
+             const unsigned *__restrict__ fx_bounds = nullptr, int fx_bits = 0,
+             const __grid_constant__ ScaFuse fz = ScaFuse{}) {
     // TV = long long: grad_value in 64-bit fixed point (deterministic mode): each lane adds VEC channels of every
     // corner contribution with scalar integer reductions, scaled by 2^(fx_bits - fx_exponent(fx_bounds)) (common.cuh);
     // non-finite bounds: nothing is scattered (the conversion then writes NaN)
@@ -155,6 +188,11 @@ msda_bwd_d32(const T *__restrict__ value, const int64_t *__restrict__ level_hw,
     // coarse levels go through msda_bwd_splat_d32, which merges them in registers, on a second stream)
     constexpr int VEC = Vec<T>::N, LANES = 32 / VEC, G = 32 / LANES;
     constexpr bool kHalfDot = std::is_same<T, bf16>::value && std::is_same<TG, bf16>::value;
+    static_assert(!kFused || (LANES == 4 && G == kFuseHeads), "the fused prep needs 16-bit value rows");
+    // fused epilogue of a one-camera row: attn, grad_attn and the packed d_offsets of its 32 samples, per row group
+    __shared__ float s_fa[kFused ? kThreads / 32 * G : 1][kFuseLP];
+    __shared__ float s_fg[kFused ? kThreads / 32 * G : 1][kFuseLP];
+    __shared__ __align__(16) uint32_t s_fo[kFused ? kThreads / 32 * G : 1][kFuseLP];
     __shared__ LevelTab tab;
     __shared__ unsigned s_skip;
     if (threadIdx.x == 0)     // levels masked for the dense path only if that kernel saw the same pyramid
@@ -199,6 +237,21 @@ msda_bwd_d32(const T *__restrict__ value, const int64_t *__restrict__ level_hw,
     const long long voff = ((long long)b * S * M + m) * 32 + sub * VEC;
     const float2 *locp = reinterpret_cast<const float2 *>(loc) + row * LP;
     const float *attp = attn + row * LP;
+    ScaRow sr;
+    float2 st = make_float2(0.f, 0.f);
+    bool single = false;                          // fused: exactly one camera sees the row's query
+    const int fgrp = (threadIdx.x >> 5) * G + grp;
+    if constexpr (kFused) {
+        live = live && sca_row(fz, row, sr);
+        if (live) {
+            st = __ldg(fz.stats + row);
+            // counted in pair_of: the per-item inv_count cannot tell one camera from none, and with bs > 1 it
+            // follows each item's own mask while the pair list follows item 0's
+            int seen = 0;
+            for (int c = 0; c < fz.ncam; ++c) seen += __ldg(fz.pair_of + (long long)c * fz.Nq + sr.q) >= 0 ? 1 : 0;
+            single = seen == 1;
+        }
+    }
 
     float g[VEC];                                 // this lane's slice of the grad_out row, fp32
     load_vec<TG, VEC>(grad_out + row * 32 + sub * VEC, g);
@@ -261,8 +314,14 @@ msda_bwd_d32(const T *__restrict__ value, const int64_t *__restrict__ level_hw,
         if (mine) {
             const int l = level_of(sm, magic);
             Hm = tab.h[l]; Wm = tab.w[l];
-            const float2 xy = __ldg(locp + sm);
-            a = __ldg(attp + sm);
+            float2 xy;
+            if constexpr (kFused) {
+                sca_loc(sr, sm, l, P, fz.Dz, Hm, Wm, xy.x, xy.y);
+                a = sca_attn(sr, sm, st.x, st.y);
+            } else {
+                xy = __ldg(locp + sm);
+                a = __ldg(attp + sm);
+            }
             c = make_corner(xy.x, xy.y, Hm, Wm);
         }
         const int enc = (c.pidx * pix) | c.dx | (c.dy << 1);
@@ -395,9 +454,43 @@ msda_bwd_d32(const T *__restrict__ value, const int64_t *__restrict__ level_hw,
             const float gx = a * (hy * (d01 - d00) + c.ly * (d11 - d10));
             const float gy = a * (hx * (d10 - d00) + c.lx * (d11 - d01));
             const long long si = row * LP + sm;
-            grad_attn[si] = ga;
-            reinterpret_cast<float2 *>(grad_loc)[si] = make_float2((float)Wm * gx, (float)Hm * gy);
+            const float glx = (float)Wm * gx, gly = (float)Hm * gy;
+            if (!kFused || !single) {
+                grad_attn[si] = ga;
+                reinterpret_cast<float2 *>(grad_loc)[si] = make_float2(glx, gly);
+            } else {
+                // sca_prep_bwd_m8 with one camera: its sums start at 0 (0 + x only differs from x for x = -0)
+                s_fa[fgrp][sm] = a;
+                s_fg[fgrp][sm] = 0.f + ga;
+                s_fo[fgrp][sm] = pack_bf16x2(__fdiv_rn(0.f + glx, (float)Wm), __fdiv_rn(0.f + gly, (float)Hm));
+            }
         }
+    }
+    if constexpr (kFused) {
+        // d_raw of a one-camera row, in the prep kernel's partition: lane `sub` owns samples [8 sub, 8 sub + 8)
+        __syncwarp();
+        float fa[8], fg[8], dot = 0.f;
+        const bool fin = live && single;
+#pragma unroll
+        for (int i = 0; i < 8; ++i) {
+            fa[i] = fin ? s_fa[fgrp][8 * sub + i] : 0.f;
+            fg[i] = fin ? s_fg[fgrp][8 * sub + i] : 0.f;
+            dot += fa[i] * fg[i];
+        }
+        dot = quad_sum(dot);
+        if (fin) {
+            bf16 *dr = fz.d_raw + sr.raw_row * (kFuseHeads * kFuseLP * 3);
+#pragma unroll
+            for (int i = 0; i < 8; ++i) fg[i] = fa[i] * (fg[i] - dot);
+            *reinterpret_cast<uint4 *>(dr + kFuseHeads * kFuseLP * 2 + m * kFuseLP + 8 * sub) =
+                make_uint4(pack_bf16x2(fg[0], fg[1]), pack_bf16x2(fg[2], fg[3]), pack_bf16x2(fg[4], fg[5]),
+                           pack_bf16x2(fg[6], fg[7]));
+            const uint4 *so = reinterpret_cast<const uint4 *>(&s_fo[fgrp][8 * sub]);
+            uint4 *dof = reinterpret_cast<uint4 *>(dr + m * kFuseLP * 2 + 16 * sub);
+            dof[0] = so[0];
+            dof[1] = so[1];
+        }
+        __syncwarp();
     }
     }
 }
@@ -549,15 +642,27 @@ static int check_dims(const char *who, int B, int S, int M, int D, int Q, int L,
 template <typename T, typename TO>
 static int launch_fwd(const char *who, const void *value, const int64_t *hw, const int64_t *ls,
                       const float *loc, const float *attn, void *out, const int *row_map, int S,
-                      int M, int D, int Q, int L, int P, long long rows, cudaStream_t st) {
+                      int M, int D, int Q, int L, int P, long long rows, cudaStream_t st,
+                      const ScaFuse *fz = nullptr) {
     if (D == 32) {
         constexpr int G = Vec<T>::N;      // rows per warp == channels per lane (4 or 8)
         const int iters = pick_iters(rows, G);
         const long long per_block = (long long)(kThreads / 32) * G * iters;
         const unsigned grid = (unsigned)((rows + per_block - 1) / per_block);
-        msda_fwd_d32<T, TO><<<grid, kThreads, 0, st>>>((const T *)value, hw, ls, loc, attn, (TO *)out,
-                                                       row_map, S, M, Q, L, P, (65536 + P - 1) / P, iters,
-                                                       rows);
+        if (fz) {
+            if constexpr (std::is_same<T, bf16>::value && std::is_same<TO, bf16>::value)
+                msda_fwd_d32<T, TO, true><<<grid, kThreads, 0, st>>>((const T *)value, hw, ls, nullptr, nullptr, (TO *)out,
+                                                                     row_map, S, M, Q, L, P, (65536 + P - 1) / P, iters,
+                                                                     rows, *fz);
+            else
+                return fail("%s: the fused prep needs bf16 value and output", who);
+        } else {
+            msda_fwd_d32<T, TO><<<grid, kThreads, 0, st>>>((const T *)value, hw, ls, loc, attn, (TO *)out,
+                                                           row_map, S, M, Q, L, P, (65536 + P - 1) / P, iters,
+                                                           rows);
+        }
+    } else if (fz) {
+        return fail("%s: the fused prep needs head_dim 32", who);
     } else {
         const unsigned grid = (unsigned)((rows + kThreads / 32 - 1) / (kThreads / 32));
         msda_fwd_generic<T, TO><<<grid, kThreads, 0, st>>>((const T *)value, hw, ls, loc, attn,
@@ -594,7 +699,7 @@ int dense_coarse_backward(const char *who, const int64_t *hw_dev, const int64_t 
                           const float *loc, const float *attn, const void *grad_out, float *grad_value,
                           const int32_t *map_range, int NB, int S, int M, int L, int P, cudaStream_t st,
                           unsigned *handled, HostLevels *host_levels, int first_level, unsigned need_mask,
-                          int gv_S, int gv_base);                                      // msda_dense.cu
+                          int gv_S, int gv_base, int loc_level0);                      // msda_dense.cu
 
 // second stream + events for the hybrid backward (created by bevf_msda_set_backward_mode(2), i.e. outside any
 // stream capture; the fork / join below is capturable)
@@ -659,7 +764,9 @@ static int launch_bwd(const char *who, const void *value, const int64_t *hw, con
                       float *ga, const int *row_map, const int *order, int S, int M, int D, int Q,
                       int L, int P, long long rows, cudaStream_t st, unsigned done_levels = 0,
                       const HostLevels *host_levels = nullptr, bool gv_f16 = false,
-                      const MixedGv *mixed = nullptr, const FxGv *fx = nullptr) {
+                      const MixedGv *mixed = nullptr, const FxGv *fx = nullptr, const ScaFuse *fz = nullptr) {
+    if (fz && (fx || gv_f16 || !mixed || !mixed->gv16))
+        return fail("%s: the fused prep runs with mixed grad_value accumulation only", who);
     HostLevels hl;
     if (host_levels) hl = *host_levels; else memset(&hl, 0, sizeof(hl));
     if (fx) {
@@ -705,6 +812,16 @@ static int launch_bwd(const char *who, const void *value, const int64_t *hw, con
             const int iters = pick_iters(rows, G);
             const long long per_block = (long long)(kThreads / 32) * G * iters;
             const unsigned grid = (unsigned)((rows + per_block - 1) / per_block);
+            if (fz) {
+                if constexpr (std::is_same<TG, bf16>::value)
+                    msda_bwd_d32<T, TG, true, float, true><<<grid, kThreads, 0, st>>>(
+                        (const T *)value, hw, ls, nullptr, nullptr, (const TG *)go, gv, gl, ga, row_map, S, M, Q, L, P,
+                        (65536 + P - 1) / P, iters, rows, done_levels, hl, mixed->amax, mixed->gv16, mixed->mask,
+                        mixed->side_start, mixed->S_side, nullptr, 0, *fz);
+                else
+                    return fail("%s: the fused prep needs a bf16 grad_out", who);
+                return check_launch(who);
+            }
             msda_bwd_d32<T, TG, true><<<grid, kThreads, 0, st>>>((const T *)value, hw, ls, loc, attn, (const TG *)go, gv, gl, ga,
                                                                row_map, S, M, Q, L, P, (65536 + P - 1) / P, iters, rows,
                                                                done_levels, hl, mixed->amax, mixed->gv16, mixed->mask, mixed->side_start,
@@ -765,15 +882,22 @@ static int launch_bwd(const char *who, const void *value, const int64_t *hw, con
 static int msda_forward_impl(const char *who, const void *value, int value_dtype,
                              const int64_t *level_hw, const int64_t *level_start, const float *loc,
                              const float *attn, void *out, int out_dtype, const int *row_map, int B,
-                             int S, int M, int D, int Q, int L, int P, void *stream) {
+                             int S, int M, int D, int Q, int L, int P, void *stream,
+                             const ScaFuse *fz = nullptr) {
     if (int e = check_dims(who, B, S, M, D, Q, L, P)) return e;
     const long long rows = (row_map ? 1ll : (long long)B) * Q * M;
     if (rows == 0) return 0;
-    if (!value || !level_hw || !level_start || !loc || !attn || !out)
+    if (!value || !level_hw || !level_start || ((!loc || !attn) && !fz) || !out)
         return fail("%s: null pointer argument", who);
     if (!aligned16(value) || !aligned16(loc) || !aligned16(attn) || !aligned16(out))
         return fail("%s: device pointers must be 16-byte aligned", who);
     cudaStream_t st = (cudaStream_t)stream;
+    if (fz) {
+        if (value_dtype != BEVF_DTYPE_BF16 || out_dtype != BEVF_DTYPE_BF16)
+            return fail("%s: the fused prep needs bf16 value and output", who);
+        return launch_fwd<bf16, bf16>(who, value, level_hw, level_start, nullptr, nullptr, out, row_map, S, M, D, Q, L, P,
+                                      rows, st, fz);
+    }
     if (value_dtype == BEVF_DTYPE_F16) {
         // fp16 value: fp16 or fp32 output
         if (out_dtype == BEVF_DTYPE_F16) return launch_fwd<__half, __half>(who, value, level_hw, level_start, loc, attn, out, row_map, S, M, D, Q, L, P, rows, st);
@@ -796,17 +920,25 @@ static int msda_backward_impl(const char *who, const void *value, int value_dtyp
                               const int *row_map, const int *order, int B, int S, int M, int D, int Q,
                               int L, int P, void *stream, unsigned done_levels = 0,
                               const HostLevels *host_levels = nullptr, bool gv_f16 = false,
-                              const MixedGv *mixed = nullptr, const FxGv *fx = nullptr) {
+                              const MixedGv *mixed = nullptr, const FxGv *fx = nullptr,
+                              const ScaFuse *fz = nullptr) {
     if (int e = check_dims(who, B, S, M, D, Q, L, P)) return e;
     const long long rows = (row_map ? 1ll : (long long)B) * Q * M;
     if (rows == 0) return 0;
-    if (!value || !level_hw || !level_start || !loc || !attn || !grad_out || !grad_value ||
+    if (!value || !level_hw || !level_start || ((!loc || !attn) && !fz) || !grad_out || !grad_value ||
         !grad_loc || !grad_attn)
         return fail("%s: null pointer argument", who);
     if (!aligned16(value) || !aligned16(loc) || !aligned16(attn) || !aligned16(grad_out) ||
         !aligned16(grad_value) || !aligned16(grad_loc) || !aligned16(grad_attn))
         return fail("%s: device pointers must be 16-byte aligned", who);
     cudaStream_t st = (cudaStream_t)stream;
+    if (fz) {
+        if (value_dtype != BEVF_DTYPE_BF16 || grad_out_dtype != BEVF_DTYPE_BF16)
+            return fail("%s: the fused prep needs bf16 value and grad_out", who);
+        return launch_bwd<bf16, bf16>(who, value, level_hw, level_start, nullptr, nullptr, grad_out, grad_value, grad_loc,
+                                      grad_attn, row_map, order, S, M, D, Q, L, P, rows, st, done_levels, host_levels,
+                                      gv_f16, mixed, fx, fz);
+    }
     if (value_dtype == BEVF_DTYPE_F16) {
         // fp16 value: fp16 or fp32 grad_out; grad_value stays fp32 (or fixed point)
         if (grad_out_dtype == BEVF_DTYPE_F16) return launch_bwd<__half, __half>(who, value, level_hw, level_start, loc, attn, grad_out, grad_value, grad_loc, grad_attn, row_map, order, S, M, D, Q, L, P, rows, st, done_levels, host_levels, gv_f16, mixed, fx);
@@ -949,7 +1081,7 @@ extern "C" int bevf_msda_rows_backward_dense(const void *value, int value_dtype,
             ds = g_side_stream;
         }
         const int e = dense_coarse_backward(who, level_hw, level_start, level_hw_host, loc, attn, grad_out, grad_value,
-                                            map_range, B, S, M, L, P, ds, &handled, &hl, 0, 0u, S, 0);
+                                            map_range, B, S, M, L, P, ds, &handled, &hl, 0, 0u, S, 0, 0);
         if (join) cudaEventRecord(join, g_side_stream);
         if (e) {
             if (join) cudaStreamWaitEvent(st, join, 0);
@@ -985,7 +1117,8 @@ static int rows_backward_mixed_impl(const char *who, const void *value, int valu
                                     void *grad_value_fine_f16, float *grad_value_side, const uint32_t *amax_bits,
                                     int num_f16_levels, int first_dense_level, float *grad_loc, float *grad_attn,
                                     const int32_t *row_map, const int32_t *group_order, const int32_t *map_range,
-                                    int B, int S, int M, int D, int R, int L, int P, void *stream) {
+                                    int B, int S, int M, int D, int R, int L, int P, void *stream,
+                                    const ScaFuse *fz = nullptr) {
     if (!row_map && R > 0) return fail("%s: row_map is null", who);
     if (!level_hw_host || !grad_value_fine_f16 || !grad_value_side || !amax_bits)
         return fail("%s: null pointer argument", who);
@@ -1016,8 +1149,12 @@ static int rows_backward_mixed_impl(const char *who, const void *value, int valu
     unsigned dense_levels = 0;                       // levels whose grad_value the dense kernel produced
     cudaEvent_t join = nullptr;
     const int mode = map_range ? mixed_dense_mode() : 0;
-    if (mode != 0 && R > 0 && grad_out_dtype == BEVF_DTYPE_BF16 && aligned16(loc) && aligned16(attn) &&
-        aligned16(grad_out)) {
+    // fused prep: the dense kernel reads the coarse samples the forward stored (levels [coarse_from, L))
+    const float *dloc = fz ? reinterpret_cast<const float *>(fz->coarse_loc) : loc;
+    const float *dattn = fz ? fz->coarse_attn : attn;
+    const int loc_level0 = fz ? fz->coarse_from : 0;
+    if (mode != 0 && R > 0 && grad_out_dtype == BEVF_DTYPE_BF16 && aligned16(dloc) && aligned16(dattn) &&
+        aligned16(grad_out) && dloc && dattn && loc_level0 <= first_dense_level) {
         cudaStream_t ds = st;
         if (mode == 2 && !g_side_stream) {
             // the library default creates its stream lazily, never inside a stream capture (a captured call without
@@ -1037,9 +1174,9 @@ static int rows_backward_mixed_impl(const char *who, const void *value, int valu
         // leaves them all to the reduction path (no level is split between the two)
         const unsigned suffix = ((1u << L) - 1u) & ~((1u << first_dense_level) - 1u);
         HostLevels dhl;
-        const int e = dense_coarse_backward(who, level_hw, level_start, level_hw_host, loc, attn, grad_out,
+        const int e = dense_coarse_backward(who, level_hw, level_start, level_hw_host, dloc, dattn, grad_out,
                                             grad_value_side, map_range, B, S, M, L, P, ds, &dense_levels, &dhl,
-                                            first_dense_level, suffix, mx.S_side, mx.side_start);
+                                            first_dense_level, suffix, mx.S_side, mx.side_start, loc_level0);
         if (join) cudaEventRecord(join, g_side_stream);
         if (e) {
             if (join) cudaStreamWaitEvent(st, join, 0);
@@ -1048,7 +1185,7 @@ static int rows_backward_mixed_impl(const char *who, const void *value, int valu
     }
     const int e = msda_backward_impl(who, value, value_dtype, level_hw, level_start, loc, attn, grad_out, grad_out_dtype,
                                      grad_value_side, grad_loc, grad_attn, row_map, group_order, B, S, M, D, R, L, P,
-                                     stream, dense_levels, &hl, false, &mx);
+                                     stream, dense_levels, &hl, false, &mx, nullptr, fz);
     if (join) cudaStreamWaitEvent(st, join, 0);
     return e;
 }
@@ -1080,6 +1217,79 @@ extern "C" int bevf_msda_rows_backward_mixed_dense(const void *value, int value_
                                     grad_out_dtype, grad_value_fine_f16, grad_value_side, amax_bits, num_f16_levels,
                                     first_dense_level, grad_loc, grad_attn, row_map, nullptr, map_range, B, S, M, D, R,
                                     L, P, stream);
+}
+
+// ---- SpatialCrossAttention's sampler with the sampling-point prep fused in (ScaFuse, msda_common.cuh) ----------
+static int sca_fuse_args(const char *who, const float *raw, const float *ref_cam, const int32_t *pair_q,
+                         const int32_t *pair_cam, const int32_t *pair_of, const float *stats, const float *coarse_loc,
+                         const float *coarse_attn, int coarse_from, int M, int D, int R, int L, int P, int bs, int Nq,
+                         int pairs, int Dz, int ncam, ScaFuse &fz) {
+    if (M != kFuseHeads || D != 32 || L * P != kFuseLP)
+        return fail("%s: 8 heads, head_dim 32 and num_levels * num_points == 32 only", who);
+    if (bs <= 0 || Nq <= 0 || pairs < 0 || (long long)bs * pairs != R || Dz <= 0 || P % Dz != 0 || ncam <= 0 ||
+        ncam > 16)
+        return fail("%s: bad dimension (rows = bs * pairs, num_points a multiple of the Z anchors, ncam <= 16)", who);
+    if (!raw || !ref_cam || !pair_q || !pair_cam || !stats) return fail("%s: null pointer argument", who);
+    if (!aligned16(raw) || !aligned16(stats) || (reinterpret_cast<uintptr_t>(ref_cam) & 7u))
+        return fail("%s: raw and stats must be 16-byte aligned, ref_cam 8-byte aligned", who);
+    if (coarse_from < 0 || coarse_from > L || (coarse_from < L && (!coarse_loc || !coarse_attn)))
+        return fail("%s: coarse_from must be in [0, L], with coarse_loc / coarse_attn when below L", who);
+    if (!aligned16(coarse_loc) || !aligned16(coarse_attn))
+        return fail("%s: coarse_loc / coarse_attn must be 16-byte aligned", who);
+    fz.coarse_loc = const_cast<float2 *>(reinterpret_cast<const float2 *>(coarse_from < L ? coarse_loc : nullptr));
+    fz.coarse_attn = const_cast<float *>(coarse_from < L ? coarse_attn : nullptr);
+    fz.coarse_from = coarse_from;
+    fz.raw = raw;
+    fz.ref_cam = ref_cam;
+    fz.pair_q = pair_q;
+    fz.pair_cam = pair_cam;
+    fz.pair_of = pair_of;
+    fz.stats = const_cast<float2 *>(reinterpret_cast<const float2 *>(stats));
+    fz.d_raw = nullptr;
+    fz.bs = bs; fz.Nq = Nq; fz.R = pairs; fz.Dz = Dz; fz.ncam = ncam;
+    return 0;
+}
+
+extern "C" int bevf_sca_rows_forward_fused(const void *value, int value_dtype, const int64_t *level_hw,
+                                           const int64_t *level_start, const float *raw, const float *ref_cam,
+                                           const int32_t *pair_q, const int32_t *pair_cam, float *stats,
+                                           float *coarse_loc, float *coarse_attn, int coarse_from, void *out,
+                                           int out_dtype, const int32_t *row_map, int B, int S, int M, int D, int R,
+                                           int L, int P, int bs, int Nq, int pairs, int Dz, int ncam, void *stream) {
+    const char *who = "bevf_sca_rows_forward_fused";
+    if (!row_map && R > 0) return fail("%s: row_map is null", who);
+    if (R == 0) return 0;
+    ScaFuse fz;
+    if (int e = sca_fuse_args(who, raw, ref_cam, pair_q, pair_cam, nullptr, stats, coarse_loc, coarse_attn,
+                              coarse_from, M, D, R, L, P, bs, Nq, pairs, Dz, ncam, fz))
+        return e;
+    return msda_forward_impl(who, value, value_dtype, level_hw, level_start, nullptr, nullptr, out, out_dtype, row_map,
+                             B, S, M, D, R, L, P, stream, &fz);
+}
+
+extern "C" int bevf_sca_rows_backward_fused(const void *value, int value_dtype, const int64_t *level_hw,
+                                            const int64_t *level_start, const int32_t *level_hw_host, const float *raw,
+                                            const float *stats, const float *coarse_loc, const float *coarse_attn,
+                                            int coarse_from, const float *ref_cam, const int32_t *pair_q,
+                                            const int32_t *pair_cam, const int32_t *pair_of, const void *grad_out,
+                                            int grad_out_dtype, void *grad_value_fine_f16, float *grad_value_side,
+                                            const uint32_t *amax_bits, int num_f16_levels, int first_dense_level,
+                                            float *grad_loc, float *grad_attn, void *d_raw, const int32_t *row_map,
+                                            const int32_t *map_range, int B, int S, int M, int D, int R, int L, int P,
+                                            int bs, int Nq, int pairs, int Dz, int ncam, void *stream) {
+    const char *who = "bevf_sca_rows_backward_fused";
+    if (R == 0) return 0;
+    ScaFuse fz;
+    if (int e = sca_fuse_args(who, raw, ref_cam, pair_q, pair_cam, pair_of, stats, coarse_loc, coarse_attn,
+                              coarse_from, M, D, R, L, P, bs, Nq, pairs, Dz, ncam, fz))
+        return e;
+    if (!pair_of) return fail("%s: null pointer argument", who);
+    if (!d_raw || !aligned16(d_raw)) return fail("%s: d_raw must be a 16-byte aligned bf16 buffer", who);
+    fz.d_raw = reinterpret_cast<bf16 *>(d_raw);
+    return rows_backward_mixed_impl(who, value, value_dtype, level_hw, level_start, level_hw_host, nullptr, nullptr,
+                                    grad_out, grad_out_dtype, grad_value_fine_f16, grad_value_side, amax_bits,
+                                    num_f16_levels, map_range ? first_dense_level : L, grad_loc, grad_attn, row_map,
+                                    nullptr, map_range, B, S, M, D, R, L, P, stream, &fz);
 }
 
 namespace bevf {

@@ -196,6 +196,80 @@ __device__ __forceinline__ int value_map_of(const int *row_map, long long row, i
 }
 
 
+// SpatialCrossAttention's sampling-point prep done inside the row-list sampler (bevf_sca_rows_forward_fused /
+// bevf_sca_rows_backward_fused): instead of reading loc / attn, a kernel derives every sample from the head's raw
+// offsets|logits, the row's softmax statistics and the camera-projected reference points -- with exactly the
+// operations of sca_prep_fwd_m8 (encoder_ops.cu), so the samples are bit-identical to the prep kernel's.
+// Sampler row (t, m): pair row t = b * R + r of batch item b, head m; 8 heads, L * P == 32.
+struct ScaFuse {
+    const float *raw;          // (bs * Nq, 8 * 32 * 3) fp32: per BEV query [offsets (8, L, P, 2) | logits (8, L * P)]
+    const float *ref_cam;      // (ncam, bs, Nq, Dz, 2)
+    const int *pair_q, *pair_cam, *pair_of;
+    float2 *stats;             // (bs * R * 8): softmax max and 1 / sum of every sampler row (written by the forward)
+    bf16 *d_raw;               // backward: (bs * Nq, 8 * 32 * 3) gradient of raw
+    // forward: the samples of levels [coarse_from, L) as (bs * R * 8, L - coarse_from, P) -- what the dense backward
+    // kernel reads (msda_dense.cu), in the loc / attn layout restricted to those levels; coarse_from = L: none
+    float2 *coarse_loc;
+    float *coarse_attn;
+    int coarse_from;
+    int bs, Nq, R, Dz, ncam;
+};
+constexpr int kFuseHeads = 8, kFuseLP = 32;
+
+// inputs of sampler row `row`; false for an unused pair row
+struct ScaRow {
+    const float *lg, *off;     // the head's logits / offsets in raw
+    const float2 *ref;         // reference points of (cam, b, q)
+    long long raw_row;         // b * Nq + q
+    int q;
+};
+__device__ __forceinline__ bool sca_row(const ScaFuse &fz, long long row, ScaRow &sr) {
+    const long long t = row / kFuseHeads;
+    const int m = (int)(row - t * kFuseHeads);
+    const int b = (int)(t / fz.R), r = (int)(t - (long long)b * fz.R);
+    const int q = __ldg(fz.pair_q + r), cam = __ldg(fz.pair_cam + r);
+    if (q < 0) return false;
+    sr.q = q;
+    sr.raw_row = (long long)b * fz.Nq + q;
+    const float *rq = fz.raw + sr.raw_row * (kFuseHeads * kFuseLP * 3);
+    sr.off = rq + m * kFuseLP * 2;
+    sr.lg = rq + kFuseHeads * kFuseLP * 2 + m * kFuseLP;
+    sr.ref = reinterpret_cast<const float2 *>(fz.ref_cam) + (((long long)cam * fz.bs + b) * fz.Nq + q) * fz.Dz;
+    return true;
+}
+// sample k = l * P + p of a row: loc = ref[p mod Dz] + off / (W, H)
+__device__ __forceinline__ void sca_loc(const ScaRow &sr, int k, int l, int P, int Dz, int H, int W, float &x,
+                                        float &y) {
+    const float2 o = __ldg(reinterpret_cast<const float2 *>(sr.off) + k);
+    const float2 rf = __ldg(sr.ref + (k - l * P) % Dz);
+    x = rf.x + __fdiv_rn(o.x, (float)W);
+    y = rf.y + __fdiv_rn(o.y, (float)H);
+}
+// attn of sample k from the row's softmax statistics: exp(logit - max) * (1 / sum)
+__device__ __forceinline__ float sca_attn(const ScaRow &sr, int k, float mx, float inv) {
+    return exp_rn(__ldg(sr.lg + k) - mx) * inv;
+}
+// softmax statistics of a row in sca_prep_fwd_m8's partition: lane `sub` of the row's quad holds logits
+// [8 sub, 8 sub + 8), and gets their attention weights in `a`; all 32 lanes must call it
+__device__ __forceinline__ float2 sca_row_stats(const ScaRow &sr, bool live, int sub, float (&a)[8]) {
+#pragma unroll
+    for (int i = 0; i < 8; i += 4) {
+        const float4 v = live ? __ldg(reinterpret_cast<const float4 *>(sr.lg + 8 * sub + i)) : make_float4(0.f, 0.f, 0.f, 0.f);
+        a[i] = v.x; a[i + 1] = v.y; a[i + 2] = v.z; a[i + 3] = v.w;
+    }
+    float mx = a[0];
+#pragma unroll
+    for (int i = 1; i < 8; ++i) mx = fmaxf(mx, a[i]);
+    mx = quad_max(mx);
+    float sum = 0.f;
+#pragma unroll
+    for (int i = 0; i < 8; ++i) { a[i] = exp_rn(a[i] - mx); sum += a[i]; }
+    const float inv = __frcp_rn(quad_sum(sum));
+#pragma unroll
+    for (int i = 0; i < 8; ++i) a[i] *= inv;
+    return make_float2(mx, inv);
+}
+
 template <typename T> __device__ __forceinline__ decltype(Vec<T>::v) vec_bits(const uint4 &u);
 template <> __device__ __forceinline__ uint4 vec_bits<bf16>(const uint4 &u) { return u; }
 template <> __device__ __forceinline__ float4 vec_bits<float>(const uint4 &u) {

@@ -156,13 +156,15 @@ __device__ __forceinline__ unsigned short bf16_add(unsigned short old, float x) 
 // so the scatter of up to NT - 1 further steps runs under the MMAs of the previous ones.
 // grad_value is (NB, gv_S, M, 32) and holds the pixels [gv_base, gv_base + gv_S) of every map: the whole pyramid
 // (gv_S = S, gv_base = 0), or the fp32 side buffer of the mixed accumulation (gv_base = its first pixel).
+// loc / attn hold the levels [loc_level0, L) of every row: (rows, M, L - loc_level0, P[, 2]) -- the whole pyramid, or
+// only the coarse samples the fused SCA forward stores (ScaFuse::coarse_loc, msda_common.cuh)
 template <int kTiles, int P, int NT>
 __global__ void __launch_bounds__(128 * NT + 256, 1)
 msda_bwd_dense_tc(const __grid_constant__ DenseBins bins, const int64_t *__restrict__ level_hw,
                   const int64_t *__restrict__ level_start, const float *__restrict__ loc,
                   const float *__restrict__ attn, const bf16 *__restrict__ grad_out,
                   float *__restrict__ grad_value, const int *__restrict__ map_range, int NB, int gv_S, int gv_base,
-                  int M, int L, int chunk_rows, int dbg) {
+                  int M, int L, int chunk_rows, int dbg, int loc_level0) {
     static_assert(P == 4 || P == 8, "points per level: 4 or 8");
     static_assert(kTiles == 4, "accumulator tiles per bin: 2 per issuer warpgroup");
     static_assert(NT >= 1 && NT <= 3, "scatter teams");
@@ -280,7 +282,7 @@ msda_bwd_dense_tc(const __grid_constant__ DenseBins bins, const int64_t *__restr
                 for (int i = 0; i < kMaxPass; ++i) {
                     q[i].x = q[i].y = q[i].a = 0.f;
                     if (live && on[i]) {
-                        const long long e = (((long long)r * M + m) * L + lv[i]) * P + pt;
+                        const long long e = (((long long)r * M + m) * (L - loc_level0) + lv[i] - loc_level0) * P + pt;
                         const float2 xy = dn::ldg_f2(reinterpret_cast<const float2 *>(loc) + e);
                         q[i].x = xy.x; q[i].y = xy.y; q[i].a = dn::ldg_f1(attn + e);
                     }
@@ -549,7 +551,7 @@ int dense_coarse_backward(const char *who, const int64_t *hw_dev, const int64_t 
                           const float *loc, const float *attn, const void *grad_out, float *grad_value,
                           const int32_t *map_range, int NB, int S, int M, int L, int P, cudaStream_t st,
                           unsigned *handled, HostLevels *host_levels, int first_level, unsigned need_mask,
-                          int gv_S, int gv_base) {
+                          int gv_S, int gv_base, int loc_level0) {
     *handled = 0;
     static const long max_pix = dense_env("BEVF_DENSE_MAXPIX", 8192);
     static const long tiles = dense_env("BEVF_DENSE_TILES", 4);
@@ -595,14 +597,14 @@ int dense_coarse_backward(const char *who, const int64_t *hw_dev, const int64_t 
         }
         kern<<<(unsigned)sms, 128 * teams + 256, smem, st>>>(bins, hw_dev, ls_dev, loc, attn, (const bf16 *)grad_out,
                                                            grad_value, map_range, NB, gv_S, gv_base, M, L, (int)chunk,
-                                                           (int)dbg);
+                                                           (int)dbg, loc_level0);
         return check_launch(who);
     };
     int e;
+    if (teams < 1 || teams > 3) return fail("%s: BEVF_DENSE_TEAMS must be 1, 2 or 3", who);
     if (teams == 3) e = (P == 8) ? launch(msda_bwd_dense_tc<4, 8, 3>) : launch(msda_bwd_dense_tc<4, 4, 3>);
     else if (teams == 2) e = (P == 8) ? launch(msda_bwd_dense_tc<4, 8, 2>) : launch(msda_bwd_dense_tc<4, 4, 2>);
-    else if (teams == 1) e = (P == 8) ? launch(msda_bwd_dense_tc<4, 8, 1>) : launch(msda_bwd_dense_tc<4, 4, 1>);
-    else return fail("%s: BEVF_DENSE_TEAMS must be 1, 2 or 3", who);
+    else e = (P == 8) ? launch(msda_bwd_dense_tc<4, 8, 1>) : launch(msda_bwd_dense_tc<4, 4, 1>);
     if (e) return e;
     *handled = mask;
     *host_levels = bins.hl;

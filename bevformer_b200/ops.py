@@ -722,6 +722,92 @@ class ScaPrep(Function):
         return (d_raw,) + (None,) * 10
 
 
+def sca_rows_forward_fused(value, spatial_shapes, level_start_index, raw, ref_cam, pair_q, pair_cam, row_map, bs, nq,
+                           coarse_from=None):
+    """SCA's row-list sampler reading the head's raw offsets|logits instead of loc / attn
+    (bevf_sca_rows_forward_fused): value (bs*ncam, S, 8, 32) bf16, raw (bs*Nq, 768) f32, ref_cam (ncam, bs, Nq, Dz, 2)
+    f32, pair_q / pair_cam (pairs,) int32, row_map (bs*pairs,) int32.  Returns (out (bs*pairs, 256) bf16, stats
+    (bs*pairs*8, 2) f32 -- the softmax statistics the backward recomputes the samples from --, coarse) where coarse is
+    None or, with ``coarse_from``, the samples of the levels [coarse_from, L) as (loc, attn, coarse_from): what the
+    backward's dense tensor-core kernel reads."""
+    for t, n in ((value, "value"), (raw, "raw"), (ref_cam, "ref_cam"), (pair_q, "pair_q"), (pair_cam, "pair_cam"),
+                 (row_map, "row_map")):
+        _need_cuda(t, n)
+    NB, S, M, D = value.shape
+    L = int(torch.as_tensor(spatial_shapes).shape[0])
+    P = raw.shape[1] // (3 * M * L)
+    R = row_map.numel()
+    ss, ls = _level_tensors(value, spatial_shapes, level_start_index)
+    out = torch.empty((R, M * D), device=value.device, dtype=value.dtype)
+    stats = torch.empty((R * M, 2), device=value.device, dtype=torch.float32)
+    coarse = None
+    if coarse_from is not None and 0 <= coarse_from < L:
+        nl = L - coarse_from
+        coarse = (torch.empty((R, M, nl, P, 2), device=value.device, dtype=torch.float32),
+                  torch.empty((R, M, nl, P), device=value.device, dtype=torch.float32), int(coarse_from))
+    lib = _lib.load()
+    with torch.cuda.device(value.device), _timed("msda_rows_forward", value.device, (R, L)):
+        st = lib.bevf_sca_rows_forward_fused(value.data_ptr(), _DT[value.dtype], ss.data_ptr(), ls.data_ptr(),
+                                             raw.data_ptr(), ref_cam.data_ptr(), pair_q.data_ptr(), pair_cam.data_ptr(),
+                                             stats.data_ptr(), _ptr(coarse and coarse[0]), _ptr(coarse and coarse[1]),
+                                             L if coarse is None else coarse[2], out.data_ptr(), _DT[value.dtype],
+                                             row_map.data_ptr(), NB, S, M, D, R, L, P, bs, nq, pair_q.numel(),
+                                             ref_cam.shape[3], ref_cam.shape[0], _stream_ptr(value))
+    _lib.check(st, lib)
+    return out, stats, coarse
+
+
+def sca_rows_backward_fused(value, spatial_shapes, level_start_index, level_hw_host, num_f16_levels, raw, stats,
+                            ref_cam, pair_q, pair_cam, pair_of, row_map, grad_output, bs, nq, map_range=None,
+                            first_dense_level=None, coarse=None):
+    """Backward of sca_rows_forward_fused with msda_rows_backward_mixed's grad_value accumulation (``map_range``: the
+    coarse levels from ``first_dense_level`` on through the dense tensor-core kernel, which reads the forward's
+    ``coarse`` samples; without them those levels stay on the reduction path).  Returns (grad_value as a
+    LazyGradValue, d_raw (bs*Nq, 768) bf16): the sampler finishes the d_raw rows of queries seen by one camera, the
+    finish kernel (bevf_sca_prep_backward_multi) the others from the sampler's grad_loc / grad_attn."""
+    import ctypes
+    for t, n in ((value, "value"), (raw, "raw"), (stats, "stats"), (ref_cam, "ref_cam"), (pair_of, "pair_of"),
+                 (row_map, "row_map"), (grad_output, "grad_output")):
+        _need_cuda(t, n)
+    alert_not_deterministic("sca_rows_backward_fused (grad_value summed with fp16 / fp32 atomics)")
+    NB, S, M, D = value.shape
+    L = len(level_hw_host)
+    P = raw.shape[1] // (3 * M * L)
+    R = row_map.numel()
+    if not (1 <= num_f16_levels < L):
+        raise RuntimeError("fused SCA backward: num_f16_levels does not fit the pyramid")
+    ss, ls = _level_tensors(value, spatial_shapes, level_start_index)
+    s_fine = sum(int(h) * int(w) for h, w in level_hw_host[:num_f16_levels])
+    grad_output = grad_output.contiguous()
+    # scratch of the pair rows whose query more than one camera sees (only those rows are written)
+    grad_loc = torch.empty((R, M, L, P, 2), device=value.device, dtype=torch.float32)
+    grad_attn = torch.empty((R, M, L, P), device=value.device, dtype=torch.float32)
+    d_raw = torch.empty(raw.shape, device=value.device, dtype=torch.bfloat16)
+    hw = (ctypes.c_int32 * (2 * L))(*[int(v) for hw_ in level_hw_host for v in hw_])
+    lib = _lib.load()
+    with torch.cuda.device(value.device), _timed("msda_rows_backward", value.device, (R, L)):
+        amax = abs_max_bits(grad_output)
+        fine = torch.zeros((NB, s_fine, M, D), device=value.device, dtype=torch.float16)
+        side = torch.zeros((NB, S - s_fine, M, D), device=value.device, dtype=torch.float32)
+        kd = num_f16_levels if first_dense_level is None else int(first_dense_level)
+        st = lib.bevf_sca_rows_backward_fused(value.data_ptr(), _DT[value.dtype], ss.data_ptr(), ls.data_ptr(),
+                                              ctypes.addressof(hw), raw.data_ptr(), stats.data_ptr(),
+                                              _ptr(coarse and coarse[0]), _ptr(coarse and coarse[1]),
+                                              L if coarse is None else coarse[2], ref_cam.data_ptr(),
+                                              pair_q.data_ptr(), pair_cam.data_ptr(), pair_of.data_ptr(),
+                                              grad_output.data_ptr(), _DT[grad_output.dtype], fine.data_ptr(),
+                                              side.data_ptr(), amax.data_ptr(), int(num_f16_levels), kd,
+                                              grad_loc.data_ptr(), grad_attn.data_ptr(), d_raw.data_ptr(),
+                                              row_map.data_ptr(), _ptr(map_range), NB, S, M, D, R, L, P, bs, nq,
+                                              pair_q.numel(), ref_cam.shape[3], ref_cam.shape[0], _stream_ptr(value))
+        _lib.check(st, lib)
+    st = lib.bevf_sca_prep_backward_multi(raw.data_ptr(), grad_loc.data_ptr(), grad_attn.data_ptr(), pair_of.data_ptr(),
+                                          ss.data_ptr(), d_raw.data_ptr(), BF16, bs, nq, pair_q.numel(), M, L, P,
+                                          pair_of.shape[0], _stream_ptr(value))
+    _lib.check(st, lib)
+    return LazyGradValue(value.shape, fine, side, amax), d_raw
+
+
 def tsa_prep_forward(raw, ref2d, level_hw, B, Nq, M, L, P, interleave=False):
     _need_cuda(raw, "raw")
     shape = (B * Nq * 2, M, L, P) if interleave else (B * 2, Nq, M, L, P)

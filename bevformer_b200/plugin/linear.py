@@ -325,8 +325,6 @@ class _HeadTC(Function):
     @once_differentiable
     def backward(ctx, grad_loc, grad_attn):
         x, w, raw = ctx.saved_tensors
-        has_bias, wdt, bdt = ctx.meta
-        k, n = w.shape[1], w.shape[0]
         grad_loc, grad_attn = grad_loc.contiguous(), grad_attn.contiguous()
         if ctx.kind == "sca":
             _ref_cam, pair_q, _pair_cam, pair_of, ss, bs, nq, m, l, p = ctx.prep_args
@@ -336,14 +334,71 @@ class _HeadTC(Function):
             _ref, ss, bs, nq, m, l, p, interleave = ctx.prep_args
             d_raw = ops.tsa_prep_backward(raw, grad_loc, grad_attn, ss, bs, nq, m, l, p, interleave,
                                           out_dtype=w.dtype)
-        dx = dw = db = None
-        if ctx.needs_input_grad[0]:
-            dx = ops.linear_dgrad_tc(d_raw, w).view(x.shape)
-        if ctx.needs_input_grad[1]:
-            dw, db = _wgrad(d_raw, x.reshape(-1, k), n, k, wdt, bdt if has_bias else None, ctx.arena)
-        elif has_bias and ctx.needs_input_grad[2]:
-            db = ops.colsum(d_raw).to(bdt)
-        return dx, dw, db, None, None
+        return (*_head_grads(ctx, d_raw, x, w), None, None)
+
+
+def _head_grads(ctx, d_raw, x, w):
+    """(dX, dW, db) of the offsets|logits head from its 16-bit d_raw."""
+    has_bias, wdt, bdt = ctx.meta
+    k, n = w.shape[1], w.shape[0]
+    dx = dw = db = None
+    if ctx.needs_input_grad[0]:
+        dx = ops.linear_dgrad_tc(d_raw, w).view(x.shape)
+    if ctx.needs_input_grad[1]:
+        dw, db = _wgrad(d_raw, x.reshape(-1, k), n, k, wdt, bdt if has_bias else None, ctx.arena)
+    elif has_bias and ctx.needs_input_grad[2]:
+        db = ops.colsum(d_raw).to(bdt)
+    return dx, dw, db
+
+
+class _ScaHeadSamplerTC(Function):
+    """SpatialCrossAttention's offsets|logits head and its row-list sampler with the sampling-point prep inside the
+    sampler kernels (ops.sca_rows_forward_fused): loc / attn are not stored, the backward recomputes them from
+    ``raw`` and the forward's softmax statistics -- except the samples of the coarse levels that the dense tensor-core
+    kernel takes in the backward (a quarter of them at base), which the forward writes as it computes them: that
+    kernel handles one sample per thread and would otherwise wait on the pair-list and raw loads of every
+    coefficient.  One autograd node, because the sampler backward produces d_raw in
+    bf16: as a separate consumer of the fp32 ``raw`` it would be cast back to fp32 by autograd (and then to bf16
+    again for the head's GEMMs).  ``fuse`` = (ref_cam, pair_q, pair_cam, pair_of, row_map, ss, lsi, bs, nq,
+    level_hw_host, num_f16_levels, map_range)."""
+
+    @staticmethod
+    def forward(ctx, x, weight, bias, value, fuse):
+        ref_cam, pair_q, pair_cam, _pair_of, row_map, ss, lsi, bs, nq, hw_host, nfine, map_range = fuse
+        w = weight.to(x.dtype)
+        xc = x.contiguous()
+        raw = ops.linear_tc(xc, w, bias, None, False, torch.float32).reshape(-1, w.shape[0])
+        # the levels the dense kernel takes in the backward: as SamplerRows' backward hands them to it
+        kd = None
+        if any(ctx.needs_input_grad) and map_range is not None and ops._lib.load().bevf_msda_get_dense_backward():
+            kd = ops.dense_levels_for(row_map.numel() / max(1, value.shape[0]), raw.shape[1] // (3 * 8 * len(hw_host)),
+                                      hw_host)
+            kd = None if kd is None else max(kd, nfine)
+        out, stats, coarse = ops.sca_rows_forward_fused(value, ss, lsi, raw, ref_cam, pair_q, pair_cam, row_map, bs,
+                                                        nq, coarse_from=kd)
+        ctx.save_for_backward(xc, w, raw, stats, value)
+        ctx.fuse, ctx.coarse = fuse, coarse
+        ctx.meta = (bias is not None, weight.dtype, None if bias is None else bias.dtype)
+        ctx.arena = _arena_ctx(weight, bias)
+        ctx.value_early = getattr(value, "_bevf_early", None)     # see shared_input_projections
+        return out
+
+    @staticmethod
+    @once_differentiable
+    def backward(ctx, grad_out):
+        x, w, raw, stats, value = ctx.saved_tensors
+        ref_cam, pair_q, pair_cam, pair_of, row_map, ss, lsi, bs, nq, hw_host, nfine, map_range = ctx.fuse
+        coarse = ctx.coarse
+        dense = coarse is not None and ops._lib.load().bevf_msda_get_dense_backward()
+        gv, d_raw = ops.sca_rows_backward_fused(value, ss, lsi, hw_host, nfine, raw, stats, ref_cam, pair_q, pair_cam,
+                                                pair_of, row_map, grad_out, bs, nq,
+                                                map_range=map_range if dense else None,
+                                                first_dense_level=coarse[2] if dense else None, coarse=coarse)
+        ctx.coarse = None
+        gvalue = None
+        if ctx.needs_input_grad[3] and not (ctx.value_early is not None and ctx.value_early(gv)):
+            gvalue = gv.materialize()
+        return (*_head_grads(ctx, d_raw, x, w), gvalue, None)
 
 
 def sca_sampling_head(x, weight, bias, ref_cam, pair_q, pair_cam, pair_of, ss, bs, nq, m, l, p):
@@ -354,6 +409,12 @@ def sca_sampling_head(x, weight, bias, ref_cam, pair_q, pair_cam, pair_of, ss, b
         return _HeadTC.apply(x, weight, bias, "sca", (ref_cam, pair_q, pair_cam, pair_of, ss, bs, nq, m, l, p))
     raw = linear_fp32_out(x, weight, bias).reshape(bs * nq, -1)
     return ops.ScaPrep.apply(raw, ref_cam, pair_q, pair_cam, pair_of, ss, bs, nq, m, l, p)
+
+
+def sca_head_sampler(x, weight, bias, value, fuse):
+    """Sampler output (bs*pairs, C) of SpatialCrossAttention straight from the query: the offsets|logits head and the
+    row-list sampler with the sampling-point prep fused in (_ScaHeadSamplerTC; the caller checks that it applies)."""
+    return _ScaHeadSamplerTC.apply(x, weight, bias, value, fuse)
 
 
 def tsa_sampling_head(x, weight, bias, ref, ss, bs, nq, m, l, p, interleave=False):

@@ -22,7 +22,7 @@ import torch
 import torch.nn as nn
 
 from .. import ops, precision
-from .linear import linear, sca_sampling_head, stacked_head
+from .linear import _use_tc as use_tc, linear, sca_head_sampler, sca_sampling_head, stacked_head
 from .registry import ATTENTION, _register, build_attention
 from .temporal_self_attention import _check_head_dim, ring_offsets_
 
@@ -204,6 +204,19 @@ class SpatialCrossAttention(nn.Module):
         nn.init.xavier_uniform_(self.output_proj.weight)
         nn.init.zeros_(self.output_proj.bias)
 
+    def _fused_prep(self, query, w, v, gv_mode, staged) -> bool:
+        """Whether the sampler computes the sampling points itself (plugin/linear.py::sca_head_sampler): the 16-bit
+        tensor-core head, 8 heads of 32 channels and 32 samples per head, the mixed grad_value accumulation with a
+        host pyramid that matches the value maps, outside deterministic mode (its fixed-point backward reads loc /
+        attn) and unless the staged forward or the pre-filled fp32 grad_value buffer (opt-in A/B paths of
+        ops.SamplerRows) was asked for."""
+        da = self.deformable_attention
+        return (isinstance(gv_mode, tuple) and staged is not None and not ops.deterministic()
+                and da.num_heads == 8 and v.shape[-1] == 32 and da.num_levels * da.num_points == 32
+                and use_tc(query, w) and sum(h * w_ for h, w_ in gv_mode[1]) == v.shape[1]
+                and os.environ.get("BEVF_MSDA_FWD", "plain") != "staged"
+                and os.environ.get("BEVF_AUX_FILL", "0") != "1")
+
     def attend(self, query, value, reference_points_cam, bev_mask, spatial_shapes,
                level_start_index, plan: Optional[ScaPlan] = None, level_hw_host=None, value_pre=None):
         """Everything up to and including output_proj, WITHOUT dropout / residual.
@@ -224,8 +237,6 @@ class SpatialCrossAttention(nn.Module):
             raise AssertionError("num_points must be a multiple of the pillar anchors")   # :369
         # offsets / logits once per BEV query: they do not depend on the camera (:338-341)
         w, b = da.head_weights(query)
-        loc, attn = sca_sampling_head(query, w, b, plan.ref_cam, plan.pair_q, plan.pair_cam,
-                                      plan.pair_of, ss, bs, nq, m, l, p)
         # value_proj over every camera's feature pyramid (:334), batch-major like the reference
         if value_pre is None:
             feats = value.permute(2, 0, 1, 3).reshape(bs * ncam, s, c)
@@ -242,7 +253,15 @@ class SpatialCrossAttention(nn.Module):
         gv_mode = None
         if level_hw_host is not None and len(level_hw_host) == l and v.dtype == torch.bfloat16:
             gv_mode = ops.gv_mode_for(plan.row_map.numel() / max(1, bs * ncam), p, level_hw_host)
-        out = ops.SamplerRows.apply(v, loc, attn, plan.row_map, ss, lsi, None, staged, gv_mode)   # (bs*R, C)
+        if self._fused_prep(query, w, v, gv_mode, staged):
+            # the sampling-point prep inside the sampler kernels: loc / attn never go through memory
+            fuse = (plan.ref_cam, plan.pair_q, plan.pair_cam, plan.pair_of, plan.row_map, ss, lsi, bs, nq,
+                    gv_mode[1], gv_mode[2], plan.map_range)
+            out = sca_head_sampler(query, w, b, v, fuse)                                      # (bs*R, C)
+        else:
+            loc, attn = sca_sampling_head(query, w, b, plan.ref_cam, plan.pair_q, plan.pair_cam,
+                                          plan.pair_of, ss, bs, nq, m, l, p)
+            out = ops.SamplerRows.apply(v, loc, attn, plan.row_map, ss, lsi, None, staged, gv_mode)   # (bs*R, C)
         slots = ops.ScaCombine.apply(out, plan.pair_of, plan.pair_q, plan.inv_count, bs, nq)
         return linear(slots, self.output_proj.weight, self.output_proj.bias)
 

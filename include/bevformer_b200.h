@@ -362,6 +362,47 @@ BEVF_API int bevf_sca_prep_backward(const float *raw, const float *grad_loc, con
                                     void *stream);
 
 /*
+ * SCA's row-list sampler with the sampling-point prep fused in: the kernels derive every sample's loc / attn
+ * from raw + ref_cam exactly as bevf_sca_prep_forward does (bit-identical), so loc / attn never go through
+ * memory.  8 heads, head_dim 32, L * P == 32, bf16 value / output / grad_out.
+ *   value (B, S, 8, 32) bf16 with B = bs * ncam value maps; row_map (R,) as for bevf_msda_rows_forward, R = bs * pairs
+ *   raw, ref_cam, pair_q, pair_cam as for bevf_sca_prep_forward (pairs = its R, ncam, Dz = its D)
+ *   stats (R * 8, 2) f32 out: softmax max and 1 / sum of every (pair row, head); the backward reads them
+ *   coarse_loc (R, 8, L - coarse_from, P, 2), coarse_attn (R, 8, L - coarse_from, P) f32 out: the samples of the levels
+ *   [coarse_from, L), which the backward's dense tensor-core kernel reads; coarse_from = L: none (pointers may be NULL)
+ */
+BEVF_API int bevf_sca_rows_forward_fused(const void *value, int value_dtype, const int64_t *level_hw,
+                                         const int64_t *level_start, const float *raw, const float *ref_cam,
+                                         const int32_t *pair_q, const int32_t *pair_cam, float *stats,
+                                         float *coarse_loc, float *coarse_attn, int coarse_from, void *out,
+                                         int out_dtype, const int32_t *row_map, int B, int S, int M, int D, int R,
+                                         int L, int P, int bs, int Nq, int pairs, int Dz, int ncam, void *stream);
+
+/* Backward of the above with bevf_msda_rows_backward_mixed_dense's grad_value accumulation (map_range NULL: that
+ * of bevf_msda_rows_backward_mixed without the dense kernel; the dense kernel runs only where the forward stored the
+ * samples of its levels, coarse_from <= first_dense_level).  The d_raw rows (bf16, layout of raw) of the queries
+ * seen by exactly one camera (counted in pair_of) are finished here; the other pair rows store grad_loc / grad_attn
+ * ((R, 8, L, P, 2) / (R, 8, L, P) f32 scratch) and bevf_sca_prep_backward_multi completes d_raw from them. */
+BEVF_API int bevf_sca_rows_backward_fused(const void *value, int value_dtype, const int64_t *level_hw,
+                                          const int64_t *level_start, const int32_t *level_hw_host, const float *raw,
+                                          const float *stats, const float *coarse_loc, const float *coarse_attn,
+                                          int coarse_from, const float *ref_cam, const int32_t *pair_q,
+                                          const int32_t *pair_cam, const int32_t *pair_of, const void *grad_out,
+                                          int grad_out_dtype, void *grad_value_fine_f16, float *grad_value_side,
+                                          const uint32_t *amax_bits, int num_f16_levels, int first_dense_level,
+                                          float *grad_loc, float *grad_attn, void *d_raw, const int32_t *row_map,
+                                          const int32_t *map_range, int B, int S, int M, int D, int R, int L, int P,
+                                          int bs, int Nq, int pairs, int Dz, int ncam, void *stream);
+
+/* bevf_sca_prep_backward for the queries NOT seen by exactly one camera (0 cameras: zero rows; 2+: the sum over
+ * their pair rows in camera order); the rows of one-camera queries are left as they are.  8 heads, L * P == 32,
+ * bf16 / fp16 d_raw. */
+BEVF_API int bevf_sca_prep_backward_multi(const float *raw, const float *grad_loc, const float *grad_attn,
+                                          const int32_t *pair_of, const int64_t *level_hw, void *d_raw,
+                                          int out_dtype, int B, int Nq, int R, int M, int L, int P, int ncam,
+                                          void *stream);
+
+/*
  * TSA sampling points.  replaces temporal_self_attention.py:206-229 (view, softmax over L*P per
  * queue entry, the two permute+reshape copies, offset / (W, H) + reference point).
  *   raw    (B*Nq, M*2*L*P*3) f32: [offsets (M,2,L,P,2) | logits (M,2,L*P)]
