@@ -115,6 +115,13 @@ SIGNATURES = {
                                            c_void_p]),
     "bevf_point_sampling": (c_int, [c_void_p, c_void_p, c_void_p, ctypes.c_float, ctypes.c_float,
                                     c_void_p, c_void_p] + [c_int] * 5 + [c_void_p]),
+    "bevf_attn_forward": (c_int, [c_void_p, c_int64] * 4 + [c_void_p] + [c_int] * 6
+                          + [ctypes.c_float, ctypes.c_float, ctypes.c_uint64, c_void_p, c_int, c_void_p]),
+    "bevf_attn_backward": (c_int, [c_void_p, c_int64] * 5 + [c_void_p, c_void_p] + [c_void_p, c_int64] * 3
+                           + [c_int] * 6 + [ctypes.c_float, ctypes.c_float, ctypes.c_uint64, c_void_p, c_int,
+                                            c_void_p]),
+    "bevf_attn_dropout_mask": (c_int, [c_void_p] + [c_int] * 5 + [ctypes.c_float, ctypes.c_uint64, c_void_p,
+                                                                  c_void_p]),
 }
 
 

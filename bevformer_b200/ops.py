@@ -1332,3 +1332,112 @@ class FlattenFeats(Function):
         if need[1]:
             d_level = d_level.to(ldt)
         return (d_cams, d_level, *d_feats)
+
+
+# ---------------------------------------------------------------------------------------------------
+# Grouped multi-head attention (csrc/attention.cu): the self-attention of Group DETR's decoder.
+# ---------------------------------------------------------------------------------------------------
+
+def _seq_operand(t: torch.Tensor):
+    """(tensor, row stride) of a sequence-first (N, bs, W) operand read in place: unit channel stride, rows at one
+    uniform stride (a column slice of a projection output qualifies).  Anything else is copied contiguous."""
+    if (t.dim() == 3 and t.stride(2) == 1 and t.stride(0) == t.shape[1] * t.stride(1)
+            and t.stride(1) % 8 == 0 and t.data_ptr() % 16 == 0):
+        return t, int(t.stride(1))
+    t = t.contiguous()
+    return t, int(t.shape[2])
+
+
+def attention_dropout_mask(nq, nk, bs, heads, groups, drop_p, seed, seed_base, device):
+    """Keep-mask (bs, groups, heads, nq / groups, nk / groups), uint8, that the attention kernels apply for this
+    (seed, seed_base): a test and debugging aid (the kernels regenerate it and never store it)."""
+    mask = torch.empty(bs, groups, heads, nq // groups, nk // groups, device=device, dtype=torch.uint8)
+    lib = _lib.load()
+    with torch.cuda.device(mask.device):
+        st = lib.bevf_attn_dropout_mask(mask.data_ptr(), nq, nk, bs, heads, groups, float(drop_p), seed,
+                                        _ptr(seed_base), torch.cuda.current_stream(mask.device).cuda_stream)
+    _lib.check(st, lib)
+    return mask
+
+
+class GroupAttention(Function):
+    """Block-diagonal softmax attention over sequence-first projections, head_dim 32, bf16 / fp16.
+
+    ``apply(q, k, v, heads, groups, scale, drop_p)``: q (Nq, bs, H*32), k / v (Nk, bs, H*32); query group g
+    (tokens [g*Nq/G, (g+1)*Nq/G)) attends to key group g.  With ``k`` None, ``q`` is the stacked in-projection
+    [Q | K] (Nq, bs, 2*H*32) of a self-attention and its gradient comes back as one (Nq, bs, 2*H*32) tensor, ready
+    for a single dX GEMM against the stacked weight rows.  Returns (Nq, bs, H*32) in the operands' dtype.
+    ``drop_p`` > 0 drops attention probabilities with masks regenerated in backward (``attention_dropout_mask``
+    gives them).  The backward has no atomics: its result repeats bit for bit."""
+
+    @staticmethod
+    def forward(ctx, q, k, v, heads, groups, scale, drop_p=0.0):
+        stacked = k is None
+        C = heads * 32
+        for t, name in ((q, "q"), (v, "v")) + (() if stacked else ((k, "k"),)):
+            if not t.is_cuda:
+                raise RuntimeError(f"{name} must be a CUDA tensor (bevformer_b200 has no CPU path)")
+            if t.dtype not in TC_DTYPES or t.dtype != q.dtype:
+                raise RuntimeError("group attention: q, k and v must be all bfloat16 or all float16")
+        qs, ldq = _seq_operand(q)
+        if stacked:
+            if qs.shape[2] != 2 * C:
+                raise RuntimeError("group attention: stacked [Q | K] must have 2 * heads * 32 channels")
+            ks, ldk, k_off = qs, ldq, C
+        else:
+            ks, ldk = _seq_operand(k)
+            k_off = 0
+        vs, ldv = _seq_operand(v)
+        nq, bs = qs.shape[0], qs.shape[1]
+        nk = vs.shape[0]
+        if vs.shape[2] != C or (not stacked and (ks.shape[2] != C or ks.shape[0] != nk)) or vs.shape[1] != bs:
+            raise RuntimeError("group attention: q, k, v shapes do not match (N, bs, heads * 32)")
+        out = torch.empty(nq, bs, C, device=q.device, dtype=q.dtype)
+        lse = torch.empty(bs, groups, heads, nq // max(groups, 1), device=q.device, dtype=torch.float32)
+        seed = _next_seed() if drop_p > 0.0 else 0
+        # a copy: before the first advance_seed the step key is the live counter, which a later advance changes in
+        # place; the backward must regenerate this forward's masks
+        sbase = seed_state(q.device).clone() if drop_p > 0.0 else None
+        esz = qs.element_size()
+        lib = _lib.load()
+        with torch.cuda.device(q.device):
+            st = lib.bevf_attn_forward(qs.data_ptr(), ldq, ks.data_ptr() + k_off * esz, ldk, vs.data_ptr(), ldv,
+                                       out.data_ptr(), C, lse.data_ptr(), nq, nk, bs, heads, 32, groups, float(scale),
+                                       float(drop_p), seed, _ptr(sbase), _DT[q.dtype], _stream_ptr(q))
+        _lib.check(st, lib)
+        ctx.save_for_backward(qs, None if stacked else ks, vs, out, lse)
+        ctx.meta = (stacked, ldq, ldk, k_off, ldv, heads, groups, float(scale), float(drop_p), seed)
+        ctx.sbase = sbase
+        return out
+
+    @staticmethod
+    @once_differentiable
+    def backward(ctx, dout):
+        qs, ks, vs, out, lse = ctx.saved_tensors
+        stacked, ldq, ldk, k_off, ldv, heads, groups, scale, drop_p, seed = ctx.meta
+        if stacked:
+            ks = qs
+        C = heads * 32
+        nq, bs, nk = qs.shape[0], qs.shape[1], vs.shape[0]
+        dout = dout.to(out.dtype)
+        dos, ldgo = _seq_operand(dout)
+        esz = qs.element_size()
+        if stacked:
+            dqk = torch.empty(nq, bs, 2 * C, device=qs.device, dtype=qs.dtype)
+            dq_ptr, lddq, dk_ptr, lddk = dqk.data_ptr(), 2 * C, dqk.data_ptr() + C * esz, 2 * C
+        else:
+            dq = torch.empty(nq, bs, C, device=qs.device, dtype=qs.dtype)
+            dk = torch.empty(nk, bs, C, device=qs.device, dtype=qs.dtype)
+            dq_ptr, lddq, dk_ptr, lddk = dq.data_ptr(), C, dk.data_ptr(), C
+        dv = torch.empty(nk, bs, C, device=qs.device, dtype=qs.dtype)
+        delta = torch.empty_like(lse)
+        lib = _lib.load()
+        with torch.cuda.device(qs.device):
+            st = lib.bevf_attn_backward(qs.data_ptr(), ldq, ks.data_ptr() + k_off * esz, ldk, vs.data_ptr(), ldv,
+                                        out.data_ptr(), C, dos.data_ptr(), ldgo, lse.data_ptr(), delta.data_ptr(),
+                                        dq_ptr, lddq, dk_ptr, lddk, dv.data_ptr(), C, nq, nk, bs, heads, 32, groups,
+                                        scale, drop_p, seed, _ptr(ctx.sbase), _DT[qs.dtype], _stream_ptr(qs))
+        _lib.check(st, lib)
+        if stacked:
+            return dqk, None, dv, None, None, None, None
+        return dq, dk, dv, None, None, None, None

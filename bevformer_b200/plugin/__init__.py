@@ -1,7 +1,7 @@
 """Host-side mirror of the reference's plugin interface for the BEV-encoder hot path
 (projects/mmdet3d_plugin/bevformer/modules/__init__.py:3-5 exports the same names)."""
 from .decoder import (CustomMSDeformableAttention, DetectionTransformerDecoder, DetrTransformerDecoderLayer,
-                      MultiheadAttention, inverse_sigmoid)
+                      GroupMultiheadAttention, MultiheadAttention, inverse_sigmoid)
 from .encoder import FFN, BEVFormerEncoder, BEVFormerLayer, MyCustomBaseTransformerLayer
 from .registry import (ATTENTION, FEEDFORWARD_NETWORK, TRANSFORMER_LAYER, TRANSFORMER_LAYER_SEQUENCE,
                        build_attention, build_from_cfg, build_transformer_layer,
@@ -13,7 +13,7 @@ from .transformer import (PerceptionTransformer, PerceptionTransformerBEVEncoder
                           ResNetFusion)
 
 __all__ = ["PerceptionTransformerV2", "ResNetFusion", "BEVStream", "obtain_history_bev", "PerceptionTransformer", "PerceptionTransformerBEVEncoder", "CustomMSDeformableAttention", "DetectionTransformerDecoder",
-           "DetrTransformerDecoderLayer", "MultiheadAttention", "inverse_sigmoid", "BEVFormerEncoder", "BEVFormerLayer", "MyCustomBaseTransformerLayer", "FFN",
+           "DetrTransformerDecoderLayer", "GroupMultiheadAttention", "MultiheadAttention", "inverse_sigmoid", "BEVFormerEncoder", "BEVFormerLayer", "MyCustomBaseTransformerLayer", "FFN",
            "SpatialCrossAttention", "MSDeformableAttention3D", "TemporalSelfAttention", "ScaPlan",
            "ATTENTION", "FEEDFORWARD_NETWORK", "TRANSFORMER_LAYER", "TRANSFORMER_LAYER_SEQUENCE",
            "build_attention", "build_from_cfg", "build_transformer_layer",

@@ -20,6 +20,7 @@ import torch
 import torch.nn as nn
 
 import copy
+import warnings
 
 from .. import ops, precision
 from .linear import linear, linear_fp32_out
@@ -164,6 +165,116 @@ class MultiheadAttention(nn.Module):
         return identity + self.dropout_layer(self.proj_drop(out))
 
 
+_GROUP_DROPOUT_DEFAULT = dict(type="Dropout", drop_prob=0.)
+
+
+class GroupMultiheadAttention(nn.Module):
+    """Group DETR's decoder self-attention (group_attention.py:18-162): mmcv's MultiheadAttention wrapper whose
+    ``num_query`` queries split, in training only, into ``group`` equal slices that attend only within their own
+    slice.  The BEVFormerV2 configs train 11 groups of 900 queries (9900) and evaluate one group.
+
+    Same registry name, constructor arguments, parameters (an ``nn.MultiheadAttention`` as ``self.attn`` holds
+    ``in_proj_weight/bias`` and ``out_proj``) and forward contract as the reference.  16-bit CUDA inputs with
+    head_dim 32 and no masks run the in-projection on the wgmma GEMM (one GEMM over the [W_q; W_k] rows when query
+    and key are the same tensor), the grouped attention kernel (``ops.GroupAttention``) and the out-projection on
+    the GEMM.  fp32 inputs, masks and other head sizes take the reference arithmetic on torch.
+
+    One deviation: with the deprecated ``dropout`` kwarg the reference writes ``drop_prob`` into ``dropout_layer``
+    in place, and so into its shared default dict, which then leaks into every later instance built without
+    ``dropout_layer``.  Here a dict the caller passes is updated in place as there, the default is not shared."""
+
+    def __init__(self, embed_dims, num_heads, attn_drop=0., proj_drop=0., group=1,
+                 dropout_layer=_GROUP_DROPOUT_DEFAULT, init_cfg=None, batch_first=False, **kwargs):
+        super().__init__()
+        if dropout_layer is _GROUP_DROPOUT_DEFAULT:
+            dropout_layer = dict(dropout_layer)
+        if "dropout" in kwargs:
+            warnings.warn("The arguments `dropout` in MultiheadAttention has been deprecated, now you can "
+                          "separately set `attn_drop`(float), proj_drop(float), and `dropout_layer`(dict) ",
+                          DeprecationWarning)
+            attn_drop = kwargs["dropout"]
+            dropout_layer["drop_prob"] = kwargs.pop("dropout")
+        self.init_cfg = init_cfg
+        self.embed_dims, self.num_heads, self.group, self.batch_first = embed_dims, num_heads, group, batch_first
+        self.attn = nn.MultiheadAttention(embed_dims, num_heads, attn_drop, **kwargs)
+        self.proj_drop = nn.Dropout(proj_drop)
+        if dropout_layer and dropout_layer.get("type", "Dropout") != "Dropout":
+            raise NotImplementedError(f"GroupMultiheadAttention: dropout_layer type {dropout_layer['type']!r} is not "
+                                      "supported (only 'Dropout')")
+        self.dropout_layer = nn.Dropout(dropout_layer.get("drop_prob", 0.0)) if dropout_layer else nn.Identity()
+
+    def _kernel_ok(self, query, key, attn_mask, key_padding_mask, groups):
+        a = self.attn
+        return (query.is_cuda and query.dtype in ops.TC_DTYPES and key.dtype == query.dtype
+                and attn_mask is None and key_padding_mask is None
+                and self.embed_dims == self.num_heads * 32 and a._qkv_same_embed_dim and a.bias_k is None
+                and not a.add_zero_attn and not a.batch_first and (groups == 1 or key.shape[0] == query.shape[0]))
+
+    @precision.entry("query", "key", "value", "identity", "query_pos", "key_pos")
+    def forward(self, query, key=None, value=None, identity=None, query_pos=None, key_pos=None,
+                attn_mask=None, key_padding_mask=None, **kwargs):
+        """query (num_query, bs, C) (or batch-first); returns identity + dropout_layer(proj_drop(attn)) in the same
+        layout (group_attention.py:117-162)."""
+        if "residual" in kwargs:               # mmcv's deprecated_api_warning({'residual': 'identity'})
+            warnings.warn("'residual' is deprecated in MultiheadAttention, please use 'identity' instead",
+                          DeprecationWarning)
+            identity = kwargs.pop("residual")
+        if key is None:
+            key = query
+        if value is None:
+            value = key
+        if identity is None:
+            identity = query
+        if key_pos is None and query_pos is not None:
+            if query_pos.shape == key.shape:
+                key_pos = query_pos
+            else:
+                warnings.warn(f"position encoding of key is missing in {self.__class__.__name__}.")
+        shared = key is query and key_pos is query_pos       # self-attention: Q and K projected by one GEMM
+        qin = query if query_pos is None else query + query_pos
+        kin = qin if shared else (key if key_pos is None else key + key_pos)
+        if self.batch_first:
+            qin, kin, value = qin.transpose(0, 1), kin.transpose(0, 1), value.transpose(0, 1)
+        nq, bs = qin.shape[0], qin.shape[1]
+        groups = self.group if self.training else 1
+        if self.training and (self.group <= 0 or nq % self.group):
+            raise RuntimeError(f"GroupMultiheadAttention: {nq} queries do not split into {self.group} equal groups")
+        if self._kernel_ok(qin, kin, attn_mask, key_padding_mask, groups):
+            out = self._forward_kernel(qin, kin, value, shared, groups)
+        else:
+            out = self._forward_torch(qin, kin, value, attn_mask, key_padding_mask, nq, bs)
+        if self.batch_first:
+            out = out.transpose(0, 1)
+        return identity + self.dropout_layer(self.proj_drop(out))
+
+    def _forward_kernel(self, qin, kin, value, shared, groups):
+        a, C = self.attn, self.embed_dims
+        w, b = a.in_proj_weight, a.in_proj_bias
+        bq = (lambda lo, hi: None) if b is None else (lambda lo, hi: b[lo:hi])
+        v = linear(value, w[2 * C:], bq(2 * C, 3 * C))
+        drop = a.dropout if self.training else 0.0
+        scale = float(C // self.num_heads) ** -0.5
+        if shared:
+            qk = linear(qin, w[:2 * C], bq(0, 2 * C))
+            out = ops.GroupAttention.apply(qk, None, v, self.num_heads, groups, scale, drop)
+        else:
+            q = linear(qin, w[:C], bq(0, C))
+            k = linear(kin, w[C:2 * C], bq(C, 2 * C))
+            out = ops.GroupAttention.apply(q, k, v, self.num_heads, groups, scale, drop)
+        return linear(out, a.out_proj.weight, a.out_proj.bias)
+
+    def _forward_torch(self, query, key, value, attn_mask, key_padding_mask, nq, bs):
+        """The reference's arithmetic: groups moved to the batch axis around nn.MultiheadAttention."""
+        if self.training:
+            query = torch.cat(query.split(nq // self.group, dim=0), dim=1)
+            key = torch.cat(key.split(nq // self.group, dim=0), dim=1)
+            value = torch.cat(value.split(nq // self.group, dim=0), dim=1)
+        out = self.attn(query=query, key=key, value=value, attn_mask=attn_mask, key_padding_mask=key_padding_mask)[0]
+        if self.training:
+            out = torch.cat(out.split(bs, dim=1), dim=0)
+        return out
+
+
 def _decoder_layer_cls():
     from .encoder import MyCustomBaseTransformerLayer
 
@@ -237,3 +348,4 @@ if not HAVE_MMCV:      # with a real mmcv / mmdet these two names keep their own
     _register(ATTENTION, MultiheadAttention)
     _register(TRANSFORMER_LAYER, DetrTransformerDecoderLayer)
 _register(TRANSFORMER_LAYER_SEQUENCE, DetectionTransformerDecoder)
+_register(ATTENTION, GroupMultiheadAttention)

@@ -65,9 +65,16 @@ def entry(*activations):
             first = next((t for a in acts for t in (a if isinstance(a, (list, tuple)) else (a,))
                           if torch.is_tensor(t)), None)
             dt, amp_off = entered(self, first)
+            done = {}      # an activation passed under several names (self-attention: key is query) stays one tensor
             for n in activations:
                 if n in bound.arguments:
-                    bound.arguments[n] = cast(bound.arguments[n], dt)
+                    a = bound.arguments[n]
+                    if torch.is_tensor(a):
+                        if id(a) not in done:
+                            done[id(a)] = (a, cast(a, dt))
+                        bound.arguments[n] = done[id(a)][1]
+                    else:
+                        bound.arguments[n] = cast(a, dt)
             with amp_off:
                 return fwd(*bound.args, **bound.kwargs)
         return wrapper

@@ -610,6 +610,43 @@ BEVF_API int bevf_linear_wgrad_into_dt(const void *dy, const void *x, float *dw,
                                        int64_t workspace_bytes, int64_t M, int N, int K, int dtype,
                                        void *stream);
 
+/*
+ * Grouped ("block-diagonal") multi-head softmax attention, head_dim 32, bf16 / fp16 storage (dtype), fp32
+ * accumulation.  Replaces the split / cat along the batch axis around nn.MultiheadAttention in
+ * GroupMultiheadAttention.forward (projects/mmdet3d_plugin/bevformer/modules/group_attention.py:117-162): the
+ * `groups` equal slices of nq queries each attend only to the same slice of the nk keys.
+ *
+ * Layout (sequence-first, read and written in place): element (token t, batch b, head h, channel c) of an operand X
+ * with row stride ldx (elements, multiple of 8, >= heads * 32) is X[(t * bs + b) * ldx + h * 32 + c].  Q, K, V and
+ * their gradients each have their own pointer and stride, so [Q | K] may be one (N, bs, 2C) buffer.
+ *
+ * bevf_attn_forward writes out (nq, bs, ldo) and lse (bs, groups, heads, nq / groups), the natural-log log-sum-exp of
+ * the scaled scores in fp32.  drop_p > 0 drops attention probabilities (inverted dropout, torch's
+ * nn.MultiheadAttention semantics; the normaliser uses the undropped probabilities).  The keep bits come from
+ * Philox4x32-10 keyed by seed + *seed_base (seed_base may be NULL; a device word so CUDA-graph replays draw new
+ * masks) and the indices (b, group, head, query, key); nothing is stored.
+ *
+ * bevf_attn_backward writes dq, dk, dv (fully overwritten, same layout) from the forward's out and lse and the
+ * output gradient.  It runs two passes without atomics (queries outer for dQ and D = rowsum(dO * O), written to
+ * delta (bs, groups, heads, nq / groups) fp32 scratch; keys outer for dK and dV), so the result repeats bit for bit.
+ * seed, seed_base and drop_p must be the forward's.
+ *
+ * Other head dims and fp32 storage are not kernel cases and return an error.
+ */
+BEVF_API int bevf_attn_forward(const void *q, int64_t ldq, const void *k, int64_t ldk, const void *v, int64_t ldv,
+                               void *out, int64_t ldo, float *lse, int nq, int nk, int bs, int heads, int head_dim,
+                               int groups, float scale, float drop_p, uint64_t seed, const uint64_t *seed_base,
+                               int dtype, void *stream);
+BEVF_API int bevf_attn_backward(const void *q, int64_t ldq, const void *k, int64_t ldk, const void *v, int64_t ldv,
+                                const void *out, int64_t ldo, const void *grad_out, int64_t ldgo, const float *lse,
+                                float *delta, void *dq, int64_t lddq, void *dk, int64_t lddk, void *dv, int64_t lddv,
+                                int nq, int nk, int bs, int heads, int head_dim, int groups, float scale, float drop_p,
+                                uint64_t seed, const uint64_t *seed_base, int dtype, void *stream);
+/* Test and debugging aid: the keep-mask (1 = kept) that bevf_attn_forward / _backward apply for these arguments,
+ * as uint8 (bs, groups, heads, nq / groups, nk / groups). */
+BEVF_API int bevf_attn_dropout_mask(uint8_t *mask, int nq, int nk, int bs, int heads, int groups, float drop_p,
+                                    uint64_t seed, const uint64_t *seed_base, void *stream);
+
 #ifdef __cplusplus
 }
 #endif
