@@ -122,6 +122,9 @@ SIGNATURES = {
                                             c_void_p]),
     "bevf_attn_dropout_mask": (c_int, [c_void_p] + [c_int] * 5 + [ctypes.c_float, ctypes.c_uint64, c_void_p,
                                                                   c_void_p]),
+    "bevf_ego_motion": (c_int, [c_void_p, c_void_p, c_int, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int]
+                        + [ctypes.c_double] * 4 + [c_int, c_void_p]),
+    "bevf_rotate_bev": (c_int, [c_void_p, c_int, c_int64, c_int64, c_void_p, c_void_p] + [c_int] * 5 + [c_void_p]),
 }
 
 

@@ -1277,6 +1277,84 @@ def relu_dropout_backward(dy, h, p):
     return out
 
 
+# ---------------------------------------------------------------------------------------------------
+# Device-resident ego-motion (csrc/ego_motion.cu): the per-frame shift / rotation / CAN-bus block of
+# PerceptionTransformer.get_bev_features without host arithmetic.
+# ---------------------------------------------------------------------------------------------------
+EGO_DELTAS, EGO_CONTINUE, EGO_NEW_SCENE = 0, 1, 2
+
+
+def ego_state(device) -> torch.Tensor:
+    """An empty stream-state block for ``ego_motion`` (previous position (3 doubles), previous angle, has-history
+    word): int64[5] zeros; ``state.view(torch.float64)[:4]`` reads the doubles."""
+    return torch.zeros(5, device=device, dtype=torch.int64)
+
+
+def ego_motion(can_bus, bev_h, bev_w, grid_length, rotate_center, use_shift, out_dtype, state=None,
+               mode=EGO_DELTAS):
+    """can_bus (bs, 18) float64 CUDA -> (shift (bs, 2) f32, rot (bs, 6) f32, can_bus_mlp_in (bs, 18) out_dtype);
+    see bevf_ego_motion in the header.  ``out_dtype`` is the dtype the host path's ``bev_queries.new_tensor`` would
+    round to.  With ``state`` (``ego_state``) and a stream mode, sample 0's absolute position / angle are turned
+    into deltas on the device and the state is advanced.  No host synchronisation."""
+    _need_cuda(can_bus, "can_bus")
+    if can_bus.dtype != torch.float64 or can_bus.dim() != 2 or can_bus.shape[1] != 18:
+        raise RuntimeError("can_bus must be a (bs, 18) float64 tensor")
+    if out_dtype not in _DT:
+        raise RuntimeError("ego_motion: float32, bfloat16 or float16 only")
+    if mode != EGO_DELTAS:
+        if state is None:
+            raise RuntimeError("ego_motion: a stream mode needs the state block")
+        _need_cuda(state, "state")
+        if state.dtype != torch.int64 or state.numel() != 5:
+            raise RuntimeError("ego_motion: state must come from ops.ego_state()")
+    bs, dev = can_bus.shape[0], can_bus.device
+    shift = torch.empty((bs, 2), device=dev, dtype=torch.float32)
+    rot = torch.empty((bs, 6), device=dev, dtype=torch.float32)
+    mlp_in = torch.empty((bs, 18), device=dev, dtype=out_dtype)
+    lib = _lib.load()
+    with torch.cuda.device(dev):
+        st = lib.bevf_ego_motion(can_bus.data_ptr(), _ptr(state) if mode != EGO_DELTAS else 0, int(mode),
+                                 shift.data_ptr(), rot.data_ptr(), mlp_in.data_ptr(), _DT[out_dtype], bs,
+                                 int(bev_h), int(bev_w), float(grid_length[0]), float(grid_length[1]),
+                                 float(rotate_center[0]), float(rotate_center[1]), int(bool(use_shift)),
+                                 _stream_ptr(can_bus))
+    _lib.check(st, lib)
+    return shift, rot, mlp_in
+
+
+def rotate_bev(prev_bev, rot, bev_h, bev_w, out_dtype=None):
+    """prev_bev (bs, Nq, C) or (Nq, bs, C) (any strides with contiguous channels; a second dimension of Nq means
+    batch-first, as in get_bev_features) rotated through the grid rows ``rot`` (bs, 6) of ``ego_motion``:
+    (Nq, bs, C) in ``out_dtype`` (default: prev_bev's), one gather pass (bevf_rotate_bev).  No gradient."""
+    if not prev_bev.is_cuda:
+        raise RuntimeError("prev_bev must be a CUDA tensor (bevformer_b200 has no CPU path)")
+    out_dtype = out_dtype or prev_bev.dtype
+    if prev_bev.dtype not in _DT or out_dtype not in _DT:
+        raise RuntimeError("rotate_bev: float32, bfloat16 or float16 only")
+    if prev_bev.requires_grad and torch.is_grad_enabled():
+        raise RuntimeError("rotate_bev has no backward: pass prev_bev without gradient")
+    nq = bev_h * bev_w
+    if prev_bev.dim() != 3 or nq not in prev_bev.shape[:2]:
+        raise RuntimeError("prev_bev must be (bs, bev_h*bev_w, C) or (bev_h*bev_w, bs, C)")
+    if prev_bev.shape[1] == nq:
+        prev_bev = prev_bev.permute(1, 0, 2)
+    C = prev_bev.shape[2]
+    if prev_bev.stride(2) != 1 or prev_bev.stride(0) % 8 or prev_bev.stride(1) % 8 or prev_bev.data_ptr() % 16:
+        prev_bev = prev_bev.contiguous()
+    bs = prev_bev.shape[1]
+    _need_cuda(rot, "rot")
+    if rot.dtype != torch.float32 or tuple(rot.shape) != (bs, 6):
+        raise RuntimeError("rot must be the (bs, 6) float32 tensor of ego_motion")
+    out = torch.empty((nq, bs, C), device=prev_bev.device, dtype=out_dtype)
+    lib = _lib.load()
+    with torch.cuda.device(prev_bev.device):
+        st = lib.bevf_rotate_bev(prev_bev.data_ptr(), _DT[prev_bev.dtype], prev_bev.stride(0), prev_bev.stride(1),
+                                 rot.data_ptr(), out.data_ptr(), _DT[out_dtype], bs, int(bev_h), int(bev_w), C,
+                                 _stream_ptr(prev_bev))
+    _lib.check(st, lib)
+    return out
+
+
 class FlattenFeats(Function):
     """Multi-level camera features [(bs, ncam, C, h, w)] -> (ncam, S, bs, C) with cams_embeds and
     level_embeds added (PerceptionTransformer.get_bev_features, transformer.py:161-181): one kernel

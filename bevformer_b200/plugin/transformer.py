@@ -10,7 +10,9 @@ reference ``forward`` (transformer.py:203-289) is outside this library's scope (
 What changes underneath: the five tensor passes that build the encoder's key/value tensor become one
 kernel per pyramid level (``bevf_flatten_feats``), and the encoder is ``plugin.encoder.BEVFormerEncoder``.
 The once-per-frame host arithmetic (ego-motion shift, CAN-bus MLP on an 18-vector, torchvision's
-nearest-neighbour rotation of prev_bev) stays as the reference wrote it.
+nearest-neighbour rotation of prev_bev) stays as the reference wrote it when the metas carry ``can_bus``;
+with ``can_bus=`` passed as a (bs, 18) float64 CUDA tensor the same block runs in two kernels on the device
+(``bevf_ego_motion``, ``bevf_rotate_bev``) and the frame has no host arithmetic left.
 """
 from __future__ import annotations
 
@@ -106,6 +108,10 @@ class PerceptionTransformer(nn.Module):
                          bev_pos=None, prev_bev=None, **kwargs):
         """mlvl_feats: per level (bs, num_cams, C, h, w); bev_queries (Nq, C); bev_pos
         (bs, C, bev_h, bev_w); prev_bev (bs, Nq, C) / (Nq, bs, C) / None; kwargs carry ``img_metas``.
+        Optional ``can_bus=`` (bs, 18) float64 CUDA and ``lidar2img=`` (bs, num_cams, 4, 4) float32 CUDA replace the
+        metas' entries of the same names and select the device path (``_get_bev_features_device``): same result
+        (shift within one fp32 ulp, rotation cells equal except where the source coordinate sits on a rounding
+        boundary), no host synchronisation, prev_bev without gradient only.
         Returns bev_embed (bs, Nq, C) in the compute dtype: the autocast dtype, fp16 with ``fp16_enabled``
         (what mmcv's auto_fp16 gives), else the features' dtype (bevformer_b200.precision)."""
         dt, amp_off = precision.entered(self, mlvl_feats[0])
@@ -113,8 +119,64 @@ class PerceptionTransformer(nn.Module):
             return self._get_bev_features(precision.cast(list(mlvl_feats), dt), bev_queries, bev_h, bev_w, dt,
                                           grid_length, bev_pos, prev_bev, **kwargs)
 
+    def _get_bev_features_device(self, mlvl_feats, bev_queries, bev_h, bev_w, dt, grid_length, bev_pos, prev_bev,
+                                 can_bus, ego_state=None, ego_mode=ops.EGO_DELTAS, **kwargs):
+        """The frame with its ego-motion block on the device (selected by ``can_bus=`` being a CUDA tensor):
+        shift, rotation operand and CAN-bus MLP input come from ``bevf_ego_motion``, prev_bev is rotated by
+        ``bevf_rotate_bev``; no numpy, no ``new_tensor``, no torchvision, no host synchronisation -- with
+        ``lidar2img=`` a device tensor too, the call can be captured in a CUDA graph.  ``img_metas`` is read for
+        ``img_shape`` only and may be omitted once a call has seen it.  ``ego_state`` / ``ego_mode``: BEVStream's
+        device-side ``prev_frame_info`` (ops.ego_motion)."""
+        if not mlvl_feats[0].is_cuda:
+            raise RuntimeError("PerceptionTransformer.get_bev_features: CUDA tensors required "
+                               "(bevformer_b200 has no CPU path)")
+        if prev_bev is not None and prev_bev.requires_grad and torch.is_grad_enabled():
+            raise RuntimeError("PerceptionTransformer.get_bev_features: the device path (can_bus= as a CUDA tensor) "
+                               "takes prev_bev without gradient; for a gradient through the rotated prev_bev use "
+                               "the host path (can_bus in img_metas, no can_bus= argument)")
+        bs = mlvl_feats[0].size(0)
+        dev = mlvl_feats[0].device
+        can_bus = can_bus.to(torch.float64).reshape(bs, 18).contiguous()
+        static = self.__dict__.setdefault("_static_cache", {})
+        if kwargs.get("img_metas") is None:
+            if ("img_shape", bs) not in static:
+                raise RuntimeError("PerceptionTransformer.get_bev_features: img_metas (for img_shape) is needed on the "
+                                   "first call")
+            kwargs["img_metas"] = static["img_shape", bs]
+        else:
+            static["img_shape", bs] = [dict(img_shape=kwargs["img_metas"][0]["img_shape"])] * bs
+        shapes = tuple(tuple(f.shape[-2:]) for f in mlvl_feats)
+        if (shapes, str(dev)) not in static:           # small constant tensors: built once (a pageable host copy)
+            ss = torch.as_tensor(shapes, dtype=torch.long, device=dev)
+            static[shapes, str(dev)] = (ss, torch.cat((ss.new_zeros((1,)), ss.prod(1).cumsum(0)[:-1])))
+        spatial_shapes, level_start_index = static[shapes, str(dev)]
+
+        shift, rot, mlp_in = ops.ego_motion(can_bus, bev_h, bev_w, grid_length, self.rotate_center, self.use_shift,
+                                            bev_queries.dtype, ego_state, ego_mode)
+        if prev_bev is not None:
+            if self.rotate_prev_bev:
+                prev_bev = ops.rotate_bev(prev_bev.detach(), rot, bev_h, bev_w, dt)
+            elif prev_bev.shape[1] == bev_h * bev_w:
+                prev_bev = prev_bev.permute(1, 0, 2)
+        bev_queries = bev_queries.unsqueeze(1).repeat(1, bs, 1)
+        bev_pos = bev_pos.flatten(2).permute(2, 0, 1)
+        bev_queries = bev_queries + self.can_bus_mlp(mlp_in)[None, :, :] * self.use_can_bus
+        bev_queries, bev_pos, prev_bev = (precision.cast(t, dt) for t in (bev_queries, bev_pos, prev_bev))
+        feat_flatten = ops.FlattenFeats.apply(self.cams_embeds if self.use_cams_embeds else None,
+                                              self.level_embeds, *mlvl_feats)
+        return self.encoder(bev_queries, feat_flatten, feat_flatten, bev_h=bev_h, bev_w=bev_w, bev_pos=bev_pos,
+                            spatial_shapes=spatial_shapes, level_start_index=level_start_index, prev_bev=prev_bev,
+                            shift=shift, level_hw_host=[tuple(int(v) for v in s) for s in shapes], **kwargs)
+
     def _get_bev_features(self, mlvl_feats, bev_queries, bev_h, bev_w, dt, grid_length, bev_pos, prev_bev,
                           **kwargs):
+        can_bus = kwargs.pop("can_bus", None)
+        if torch.is_tensor(can_bus) and can_bus.is_cuda:
+            return self._get_bev_features_device(mlvl_feats, bev_queries, bev_h, bev_w, dt, grid_length, bev_pos,
+                                                 prev_bev, can_bus, **kwargs)
+        if can_bus is not None:
+            raise RuntimeError("PerceptionTransformer.get_bev_features: can_bus= must be a CUDA tensor (bs, 18); "
+                               "host values belong in img_metas[i]['can_bus']")
         img_metas = kwargs["img_metas"]
         bs = mlvl_feats[0].size(0)
         bev_queries = bev_queries.unsqueeze(1).repeat(1, bs, 1)
@@ -361,7 +423,7 @@ def patch_reference(cls):
     (which keeps its decoder ``forward``): ``patch_reference(PerceptionTransformer)`` once at import
     time of a BEVFormer checkout.  Parameter / attribute names are the reference's, so nothing else
     changes; the encoder inside is whatever the config built (the drop-in BEVFormerEncoder)."""
-    for name in ("get_bev_features", "_get_bev_features", "_shift", "_rotate_prev"):
+    for name in ("get_bev_features", "_get_bev_features", "_get_bev_features_device", "_shift", "_rotate_prev"):
         setattr(cls, name, getattr(PerceptionTransformer, name))
     return cls
 

@@ -647,6 +647,40 @@ BEVF_API int bevf_attn_backward(const void *q, int64_t ldq, const void *k, int64
 BEVF_API int bevf_attn_dropout_mask(uint8_t *mask, int nq, int nk, int bs, int heads, int groups, float drop_p,
                                     uint64_t seed, const uint64_t *seed_base, void *stream);
 
+/* ------------------------------------------------------------------------------------------------
+ * The once-per-frame ego-motion block of PerceptionTransformer.get_bev_features on the device
+ * (transformer.py:122-153, detectors/bevformer.py:254-268): no host arithmetic, so a video frame can be
+ * captured in a CUDA graph and replayed with a new CAN-bus vector.
+ *
+ * bevf_ego_motion, one launch per frame:
+ *   can_bus (bs, 18) f64 DEVICE: [0:3] ego translation, [16] ego yaw (rad), [17] yaw (deg).
+ *   mode    BEVF_EGO_DELTAS    can_bus already holds deltas to the previous frame; state is not touched (may be NULL)
+ *           BEVF_EGO_CONTINUE  can_bus is absolute: sample 0's position / angle become deltas against the state
+ *                              when it has history (zeros when it has not), then the state takes this frame's
+ *                              absolute values
+ *           BEVF_EGO_NEW_SCENE can_bus is absolute, first frame of a scene: sample 0's position / angle become
+ *                              zeros, the state takes this frame's absolute values
+ *   state   40 bytes, 8-byte aligned: double prev_pos[3]; double prev_angle; int64 has_history (all-zero = empty).
+ *   shift (bs, 2) f32 out: the BEV shift (x, y) in float64, rounded to out_dtype and widened to f32 (what
+ *           bev_queries.new_tensor(shift) followed by the encoder's .float() holds); zeros with use_shift == 0.
+ *   rot   (bs, 6) f32 out: torchvision's rotate(img, angle = can_bus[17], center) as the rows of its sampling
+ *           grid: _get_inverse_affine_matrix(center - size / 2, -angle) in float64, rounded to f32, x row divided by
+ *           0.5 * bev_w and y row by 0.5 * bev_h (_gen_affine_grid).  center = (center_x, center_y) in pixels.
+ *   can_bus_out (bs, 18) out_dtype: the CAN-bus MLP input (deltas applied).
+ *
+ * bevf_rotate_bev: out[q, b, :] = prev[src(q), b, :], or zeros where src falls outside the map; src is the
+ * nearest cell (ties to even) of grid_sample(align_corners=False) under the grid `rot` describes, computed in f32
+ * for every storage type.  prev: element (q, b, c) at prev[q * stride_q + b * stride_b + c] (so (Nq, bs, C) and
+ * (bs, Nq, C) are both read in place), in_dtype; out (Nq, bs, C) contiguous, out_dtype.  C % 8 == 0, strides % 8 == 0.
+ * Values are copied, so apart from the cast the result is exact.  out must not alias prev.
+ */
+enum bevf_ego_mode { BEVF_EGO_DELTAS = 0, BEVF_EGO_CONTINUE = 1, BEVF_EGO_NEW_SCENE = 2 };
+BEVF_API int bevf_ego_motion(const double *can_bus, void *state, int mode, float *shift, float *rot,
+                             void *can_bus_out, int out_dtype, int bs, int bev_h, int bev_w, double grid_h,
+                             double grid_w, double center_x, double center_y, int use_shift, void *stream);
+BEVF_API int bevf_rotate_bev(const void *prev, int in_dtype, int64_t stride_q, int64_t stride_b, const float *rot,
+                             void *out, int out_dtype, int bs, int bev_h, int bev_w, int C, void *stream);
+
 #ifdef __cplusplus
 }
 #endif
