@@ -988,6 +988,10 @@ using namespace bevf;
 
 static inline unsigned blocks_for(long long n, int per) { return (unsigned)((n + per - 1) / per); }
 
+// the pointers a kernel reads or writes with 16 B vectors must be 16-byte aligned (optional ones may be null);
+// scalar and atomic operands (LayerNorm's dgamma / dbeta / mean / rstd, colsum's out, inv_count) may sit anywhere
+static inline bool vec_ok(const void *p) { return p == nullptr || aligned16(p); }
+
 extern "C" int bevf_sca_prep_forward(const float *raw, const float *ref_cam, const int32_t *pair_q,
                                      const int32_t *pair_cam, const int64_t *level_hw, float *loc,
                                      float *attn, int B, int Nq, int R, int M, int L, int P, int D,
@@ -998,6 +1002,7 @@ extern "C" int bevf_sca_prep_forward(const float *raw, const float *ref_cam, con
     const long long total = (long long)B * R * M;
     if (total == 0) return 0;
     BEVF_REQUIRE(raw && ref_cam && pair_q && pair_cam && level_hw && loc && attn, who, "null pointer argument");
+    BEVF_REQUIRE(aligned16(raw) && aligned16(loc), who, "raw and loc must be 16-byte aligned");
     const int LP = L * P, pmagic = (65536 + P - 1) / P;
     cudaStream_t st = (cudaStream_t)stream;
     const unsigned wgrid = blocks_for((long long)B * R, kEThreads / 32);
@@ -1049,6 +1054,7 @@ extern "C" int bevf_sca_prep_backward(const float *raw, const float *grad_loc,
     BEVF_REQUIRE(out_dtype == BEVF_DTYPE_F32 || out_dtype == BEVF_DTYPE_BF16 || out_dtype == BEVF_DTYPE_F16, who, "unsupported dtype code");
     if ((long long)B * Nq * M == 0) return 0;
     BEVF_REQUIRE(raw && pair_of && level_hw && d_raw && (R == 0 || (grad_loc && grad_attn)), who, "null pointer argument");
+    BEVF_REQUIRE(aligned16(raw) && aligned16(d_raw), who, "raw and d_raw must be 16-byte aligned");
     cudaStream_t st = (cudaStream_t)stream;
     if (out_dtype == BEVF_DTYPE_BF16)
         return sca_prep_backward_t<bf16>(who, raw, grad_loc, grad_attn, pair_of, level_hw, (bf16 *)d_raw, B, Nq, R, M, L, P, ncam, st);
@@ -1077,6 +1083,7 @@ extern "C" int bevf_sca_prep_backward_multi(const float *raw, const float *grad_
     BEVF_REQUIRE(out_dtype == BEVF_DTYPE_BF16 || out_dtype == BEVF_DTYPE_F16, who, "bf16 or fp16 d_raw only");
     if ((long long)B * Nq == 0) return 0;
     BEVF_REQUIRE(raw && pair_of && level_hw && d_raw && (R == 0 || (grad_loc && grad_attn)), who, "null pointer argument");
+    BEVF_REQUIRE(aligned16(raw) && aligned16(d_raw), who, "raw and d_raw must be 16-byte aligned");
     cudaStream_t st = (cudaStream_t)stream;
     if (out_dtype == BEVF_DTYPE_BF16)
         sca_prep_backward_multi_t<bf16>(raw, grad_loc, grad_attn, pair_of, level_hw, (bf16 *)d_raw, B, Nq, R, L, P, ncam, st);
@@ -1093,6 +1100,7 @@ extern "C" int bevf_tsa_prep_forward(const float *raw, const float *ref2d, const
     const long long total = (long long)B * Nq * M * 2;
     if (total == 0) return 0;
     BEVF_REQUIRE(raw && ref2d && level_hw && loc && attn, who, "null pointer argument");
+    BEVF_REQUIRE(aligned16(raw) && aligned16(loc), who, "raw and loc must be 16-byte aligned");
     if (!launch_tsa_prep_m8<false, float>(raw, ref2d, nullptr, nullptr, level_hw, loc, attn, nullptr, B, Nq, M, L, P,
                                    interleave, (cudaStream_t)stream)) {
         if (interleave) return fail("%s: interleaved rows need num_heads == 8 and L*P in {2,4,8,16,32}", who);
@@ -1125,6 +1133,7 @@ extern "C" int bevf_tsa_prep_backward(const float *raw, const float *grad_loc,
     BEVF_REQUIRE(out_dtype == BEVF_DTYPE_F32 || out_dtype == BEVF_DTYPE_BF16 || out_dtype == BEVF_DTYPE_F16, who, "unsupported dtype code");
     if ((long long)B * Nq * M * 2 == 0) return 0;
     BEVF_REQUIRE(raw && grad_loc && grad_attn && level_hw && d_raw, who, "null pointer argument");
+    BEVF_REQUIRE(aligned16(raw) && aligned16(d_raw), who, "raw and d_raw must be 16-byte aligned");
     cudaStream_t st = (cudaStream_t)stream;
     if (out_dtype == BEVF_DTYPE_BF16)
         return tsa_prep_backward_t<bf16>(who, raw, grad_loc, grad_attn, level_hw, (bf16 *)d_raw, B, Nq, M, L, P, interleave, st);
@@ -1159,6 +1168,8 @@ extern "C" int bevf_layernorm_forward(const void *x, const void *residual, const
     if (rows == 0) return 0;
     BEVF_REQUIRE(x && gamma && beta && y, who, "null pointer argument");
     BEVF_REQUIRE((y_plus_pos == nullptr) == (pos == nullptr), who, "pos and y_plus_pos go together");
+    BEVF_REQUIRE(vec_ok(x) && vec_ok(residual) && vec_ok(pos) && vec_ok(y) && vec_ok(y_plus_pos), who,
+                 "x, residual, pos, y and y_plus_pos must be 16-byte aligned");
     BEVF_REQUIRE(drop_p >= 0.f && drop_p < 1.f, who, "dropout probability must be in [0, 1)");
     cudaStream_t st = (cudaStream_t)stream;
     const bool pb = param_dtype == BEVF_DTYPE_BF16;
@@ -1220,6 +1231,8 @@ static int layernorm_backward_impl(const char *who, const void *x, const void *r
     BEVF_REQUIRE(rows >= 0 && C > 0, who, "bad dimension");
     if (rows == 0) return 0;
     BEVF_REQUIRE(x && gamma && mean && rstd && dy && dx && dgamma && dbeta, who, "null pointer argument");
+    BEVF_REQUIRE(vec_ok(x) && vec_ok(residual) && vec_ok(dy) && vec_ok(dy_plus_pos) && vec_ok(dx) && vec_ok(dres), who,
+                 "x, residual, dy, dy_plus_pos, dx and dres must be 16-byte aligned");
     const long long ld2 = dy_plus_pos_ld > 0 ? (long long)dy_plus_pos_ld : (long long)C;
     BEVF_REQUIRE(ld2 >= C && ld2 % (dtype != BEVF_DTYPE_F32 ? 8 : 4) == 0, who, "bad row stride of dy_plus_pos");
     BEVF_REQUIRE(drop_p == 0.f || dres != nullptr || residual == nullptr, who, "dropout with a residual needs a separate dres buffer");
@@ -1286,6 +1299,7 @@ extern "C" int bevf_sca_combine_forward(const void *out, const int32_t *pair_of,
     BEVF_REQUIRE(B >= 0 && Nq >= 0 && R >= 0 && C > 0 && C % 8 == 0 && ncam > 0, who, "bad dimension");
     if ((long long)B * Nq == 0) return 0;
     BEVF_REQUIRE(pair_of && inv_count && slots && (R == 0 || out), who, "null pointer argument");
+    BEVF_REQUIRE(vec_ok(out) && aligned16(slots), who, "out and slots must be 16-byte aligned");
     cudaStream_t st = (cudaStream_t)stream;
     if (dtype == BEVF_DTYPE_F32) {
         sca_combine_fwd<float><<<blocks_for((long long)B * Nq * (C / 4), kEThreads), kEThreads, 0, st>>>((const float *)out, pair_of, inv_count, (float *)slots, B, Nq, R, C, ncam);
@@ -1306,6 +1320,7 @@ extern "C" int bevf_sca_combine_backward(const void *g_slots, const int32_t *pai
     BEVF_REQUIRE(B >= 0 && Nq >= 0 && R >= 0 && C > 0 && C % 8 == 0, who, "bad dimension");
     if ((long long)B * R == 0) return 0;
     BEVF_REQUIRE(g_slots && pair_q && inv_count && g_out, who, "null pointer argument");
+    BEVF_REQUIRE(aligned16(g_slots) && aligned16(g_out), who, "g_slots and g_out must be 16-byte aligned");
     cudaStream_t st = (cudaStream_t)stream;
     if (dtype == BEVF_DTYPE_F32) {
         sca_combine_bwd<float><<<blocks_for((long long)B * R * (C / 4), kEThreads), kEThreads, 0, st>>>((const float *)g_slots, pair_q, inv_count, (float *)g_out, B, Nq, R, C);
@@ -1418,6 +1433,7 @@ static int colsum_impl(const char *who, const void *x, float *out, int64_t rows,
     BEVF_REQUIRE(rows >= 0 && C > 0, who, "bad dimension");
     if (rows == 0) return 0;
     BEVF_REQUIRE(x && out, who, "null pointer argument");
+    BEVF_REQUIRE(aligned16(x), who, "x must be 16-byte aligned");
     const int vec = dtype != BEVF_DTYPE_F32 ? 8 : 4;
     BEVF_REQUIRE(dtype == BEVF_DTYPE_BF16 || dtype == BEVF_DTYPE_F16 || dtype == BEVF_DTYPE_F32, who, "unsupported dtype code");
     BEVF_REQUIRE(C % vec == 0 && C / vec <= kEThreads, who, "C must be a multiple of the vector width and <= 2048");
@@ -1466,6 +1482,7 @@ extern "C" int bevf_relu_dropout_backward(const void *dy, const void *h, void *o
     BEVF_REQUIRE(n >= 0, who, "bad dimension");
     if (n == 0) return 0;
     BEVF_REQUIRE(dy && h && out, who, "null pointer argument");
+    BEVF_REQUIRE(aligned16(dy) && aligned16(h) && aligned16(out), who, "dy, h and out must be 16-byte aligned");
     const int vec = dtype != BEVF_DTYPE_F32 ? 8 : 4;
     BEVF_REQUIRE(dtype == BEVF_DTYPE_BF16 || dtype == BEVF_DTYPE_F16 || dtype == BEVF_DTYPE_F32, who, "unsupported dtype code");
     BEVF_REQUIRE(n % vec == 0, who, "element count must be a multiple of the vector width");
@@ -1487,6 +1504,7 @@ extern "C" int bevf_dropout_inplace(void *x, int64_t n, float p, uint64_t seed, 
     BEVF_REQUIRE(p >= 0.f && p < 1.f, who, "dropout probability must be in [0, 1)");
     if (n == 0 || p == 0.f) return 0;
     BEVF_REQUIRE(x, who, "null pointer argument");
+    BEVF_REQUIRE(aligned16(x), who, "x must be 16-byte aligned");
     const int vec = dtype != BEVF_DTYPE_F32 ? 8 : 4;
     BEVF_REQUIRE(dtype == BEVF_DTYPE_BF16 || dtype == BEVF_DTYPE_F16 || dtype == BEVF_DTYPE_F32, who, "unsupported dtype code");
     BEVF_REQUIRE(n % vec == 0, who, "element count must be a multiple of the vector width");

@@ -1267,7 +1267,9 @@ def dropout_inplace_(x, p):
 def relu_dropout_backward(dy, h, p):
     """Gradient w.r.t. z of h = dropout_p(relu(z)), from the saved h alone."""
     _need_cuda(dy, "dy")
-    dy = dy.contiguous()
+    _need_cuda(h, "h")
+    if h.dtype != dy.dtype or h.numel() != dy.numel():
+        raise RuntimeError("relu_dropout_backward: h must match dy in dtype and size")
     out = torch.empty_like(dy)
     lib = _lib.load()
     with torch.cuda.device(dy.device):

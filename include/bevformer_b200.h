@@ -26,7 +26,9 @@
  *     message for the calling thread (the Python wrapper raises RuntimeError with it, which is
  *     what mmcv's TORCH_CHECK failures surface as).
  *   - tensors are dense row-major in the layouts named per function; "dtype" arguments take the
- *     BEVF_DTYPE_* codes.  Device pointers must be 16-byte aligned.
+ *     BEVF_DTYPE_* codes.  Device pointers must be 16-byte aligned; the entry points refuse a misaligned
+ *     pointer that a kernel accesses with 16 B vectors, while scalar and atomic operands (LayerNorm's mean / rstd /
+ *     dgamma / dbeta, bevf_colsum's out, inv_count) may sit at any float offset.
  *   - there is NO CPU implementation behind this ABI.
  */
 #ifndef BEVFORMER_B200_H_
