@@ -73,6 +73,9 @@ SIGNATURES = {
     "bevf_sca_prep_backward_multi": (c_int, [c_void_p] * 6 + [c_int] * 8 + [c_void_p]),
     "bevf_tsa_prep_forward": (c_int, [c_void_p] * 5 + [c_int] * 6 + [c_void_p]),
     "bevf_tsa_prep_backward": (c_int, [c_void_p] * 5 + [c_int] * 7 + [c_void_p]),
+    "bevf_query_prep_forward": (c_int, [c_void_p] * 5 + [c_int] * 7 + [c_void_p]),
+    "bevf_query_prep_backward": (c_int, [c_void_p] * 5 + [c_int] * 8 + [c_void_p]),
+    "bevf_refine_points": (c_int, [c_void_p, c_int64, c_void_p, c_void_p, c_void_p, c_int, c_int64, c_void_p]),
     "bevf_layernorm_forward": (c_int, [c_void_p] * 4 + [c_int] + [c_void_p] * 5
                                + [c_int64, c_int, ctypes.c_float, ctypes.c_float, ctypes.c_uint64, c_void_p,
                                   c_int, c_void_p]),

@@ -385,25 +385,27 @@ dropout_inplace_kernel(T *__restrict__ x, long long n_vec, float p, unsigned lon
 }
 
 // ------------------------------------------------------------------------------------------------
-// TSA sampling-point preparation.  raw row: [ offsets (M, 2, L, P, 2) | logits (M, 2, L*P) ]
-// out rows ordered (b, queue j, q): loc (B*2, Nq, M, L, P, 2), attn (B*2, Nq, M, L, P)
+// Sampling-point preparation of the query-side deformable attentions.  raw row:
+// [ offsets (M, F, L, P, 2) | logits (M, F, L*P) ] for F frames (queue entries): TSA has F = 2, the decoder's
+// CustomMSDeformableAttention F = 1.  out rows ordered (b, frame j, q): loc (B*F, Nq, M, L, P, 2),
+// attn (B*F, Nq, M, L, P)
 // ------------------------------------------------------------------------------------------------
 __global__ void __launch_bounds__(kEThreads)
 tsa_prep_fwd(const float *__restrict__ raw, const float *__restrict__ ref2d,
              const int64_t *__restrict__ level_hw, float *__restrict__ loc, float *__restrict__ attn,
-             int B, int Nq, int M, int L, int P) {
+             int B, int Nq, int M, int L, int P, int F) {
     const long long t = (long long)blockIdx.x * blockDim.x + threadIdx.x;
-    const long long total = (long long)B * Nq * M * 2;
+    const long long total = (long long)B * Nq * M * F;
     if (t >= total) return;
-    const int j = (int)(t & 1);
-    const long long t2 = t >> 1;
+    const int j = (int)(t % F);
+    const long long t2 = t / F;
     const int m = (int)(t2 % M);
     const long long bq = t2 / M;
     const int q = (int)(bq % Nq), b = (int)(bq / Nq);
-    const int LP = L * P, nout = M * 2 * LP * 3;
-    const float *off = raw + bq * nout + ((long long)m * 2 + j) * LP * 2;
-    const float *lg = raw + bq * nout + (long long)M * 2 * LP * 2 + ((long long)m * 2 + j) * LP;
-    const long long orow = (((long long)b * 2 + j) * Nq + q);
+    const int LP = L * P, nout = M * F * LP * 3;
+    const float *off = raw + bq * nout + ((long long)m * F + j) * LP * 2;
+    const float *lg = raw + bq * nout + (long long)M * F * LP * 2 + ((long long)m * F + j) * LP;
+    const long long orow = (((long long)b * F + j) * Nq + q);
     const float *rf = ref2d + orow * L * 2;
     float mx = -INFINITY;
     for (int k = 0; k < LP; ++k) mx = fmaxf(mx, lg[k]);
@@ -428,20 +430,20 @@ template <typename TO>
 __global__ void __launch_bounds__(kEThreads)
 tsa_prep_bwd(const float *__restrict__ raw, const float *__restrict__ grad_loc,
              const float *__restrict__ grad_attn, const int64_t *__restrict__ level_hw,
-             TO *__restrict__ d_raw, int B, int Nq, int M, int L, int P) {
+             TO *__restrict__ d_raw, int B, int Nq, int M, int L, int P, int F) {
     const long long t = (long long)blockIdx.x * blockDim.x + threadIdx.x;
-    const long long total = (long long)B * Nq * M * 2;
+    const long long total = (long long)B * Nq * M * F;
     if (t >= total) return;
-    const int j = (int)(t & 1);
-    const long long t2 = t >> 1;
+    const int j = (int)(t % F);
+    const long long t2 = t / F;
     const int m = (int)(t2 % M);
     const long long bq = t2 / M;
     const int q = (int)(bq % Nq), b = (int)(bq / Nq);
-    const int LP = L * P, nout = M * 2 * LP * 3;
-    const long long o_off = bq * nout + ((long long)m * 2 + j) * LP * 2;
-    const long long o_lg = bq * nout + (long long)M * 2 * LP * 2 + ((long long)m * 2 + j) * LP;
+    const int LP = L * P, nout = M * F * LP * 3;
+    const long long o_off = bq * nout + ((long long)m * F + j) * LP * 2;
+    const long long o_lg = bq * nout + (long long)M * F * LP * 2 + ((long long)m * F + j) * LP;
     const float *lg = raw + o_lg;
-    const long long orow = (((long long)b * 2 + j) * Nq + q);
+    const long long orow = (((long long)b * F + j) * Nq + q);
     const float *gl = grad_loc + (orow * M + m) * LP * 2;
     const float *ga = grad_attn + (orow * M + m) * LP;
     float mx = -INFINITY;
@@ -833,43 +835,46 @@ point_sampling_kernel(const float *__restrict__ lidar2img, PointSamplingParams p
 
 
 // ------------------------------------------------------------------------------------------------
-// Warp-cooperative TSA prep for num_heads == 8: one warp per (b, q); lane = (head m = lane / 4,
-// queue entry j = (lane / 2) % 2, half = lane % 2); a lane owns PPL = L*P/2 points; the softmax over
-// the L*P points of one (head, queue entry) reduces over the lane pair.
+// Warp-cooperative prep for num_heads == 8: 16 * F lanes per (b, q) -- one warp with TSA's F = 2 frames,
+// half a warp with the decoder's F = 1; lane = (head m, frame j, half) with half the fastest index; a lane
+// owns PPL = L*P/2 points; the softmax over the L*P points of one (head, frame) reduces over the lane pair.
 // ------------------------------------------------------------------------------------------------
 template <int PPL, bool kBackward, typename TO>
 __global__ void __launch_bounds__(kEThreads)
 tsa_prep_m8(const float *__restrict__ raw, const float *__restrict__ ref2d,
             const float *__restrict__ grad_loc, const float *__restrict__ grad_attn,
             const int64_t *__restrict__ level_hw, float *__restrict__ loc, float *__restrict__ attn,
-            TO *__restrict__ d_raw, int B, int Nq, int L, int P, int pmagic, int interleave) {
+            TO *__restrict__ d_raw, int B, int Nq, int L, int P, int pmagic, int interleave, int F) {
     constexpr int M = 8;
     __shared__ float s_w[16], s_h[16];
     if ((int)threadIdx.x < L) { s_h[threadIdx.x] = (float)level_hw[2 * threadIdx.x]; s_w[threadIdx.x] = (float)level_hw[2 * threadIdx.x + 1]; }
     __syncthreads();
-    const int lane = threadIdx.x & 31, m = lane >> 2, j = (lane >> 1) & 1, half = lane & 1;
-    const long long bq = (long long)blockIdx.x * (kEThreads / 32) + (threadIdx.x >> 5);
+    const int per_bq = 16 * F, sub = threadIdx.x & (per_bq - 1);
+    const int m = sub >> F, j = F == 2 ? (sub >> 1) & 1 : 0, half = sub & 1;
+    // the lane pair of one (head, frame): both lanes of a pair stay or leave together below
+    const unsigned pair = 3u << ((threadIdx.x & 31) & ~1);
+    const long long bq = (long long)blockIdx.x * (kEThreads / per_bq) + threadIdx.x / per_bq;
     if (bq >= (long long)B * Nq) return;
     const int q = (int)(bq % Nq), b = (int)(bq / Nq);
     const int LP = 2 * PPL, k0 = half * PPL;
-    const long long rbase = bq * (M * 2 * LP * 3);
-    const long long o_off = rbase + ((m * 2 + j) * LP + k0) * 2;
-    const long long o_lg = rbase + M * 2 * LP * 2 + (m * 2 + j) * LP + k0;
-    const long long orow = ((long long)b * 2 + j) * Nq + q;            // row of ref2d (frame-major)
+    const long long rbase = bq * (M * F * LP * 3);
+    const long long o_off = rbase + ((m * F + j) * LP + k0) * 2;
+    const long long o_lg = rbase + M * F * LP * 2 + (m * F + j) * LP + k0;
+    const long long orow = ((long long)b * F + j) * Nq + q;            // row of ref2d (frame-major)
     // output rows: frame-major (b, j, q) like the reference, or interleaved (b, q, j) so that the two
     // frames of a query are adjacent and their mean folds into the output projection
-    const long long out_row = interleave ? (((long long)b * Nq + q) * 2 + j) : orow;
+    const long long out_row = interleave ? (((long long)b * Nq + q) * F + j) : orow;
     const long long o_out = (out_row * M + m) * LP + k0;
     float a[PPL];
     ldv<PPL>(raw + o_lg, a);
     float mx = a[0];
 #pragma unroll
     for (int i = 1; i < PPL; ++i) mx = fmaxf(mx, a[i]);
-    mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, 1));
+    mx = fmaxf(mx, __shfl_xor_sync(pair, mx, 1));
     float sum = 0.f;
 #pragma unroll
     for (int i = 0; i < PPL; ++i) { a[i] = exp_rn(a[i] - mx); sum += a[i]; }
-    sum += __shfl_xor_sync(0xffffffffu, sum, 1);
+    sum += __shfl_xor_sync(pair, sum, 1);
     const float inv = __frcp_rn(sum);
 #pragma unroll
     for (int i = 0; i < PPL; ++i) a[i] *= inv;
@@ -892,7 +897,7 @@ tsa_prep_m8(const float *__restrict__ raw, const float *__restrict__ ref2d,
         float dot = 0.f;
 #pragma unroll
         for (int i = 0; i < PPL; ++i) dot += a[i] * ga[i];
-        dot += __shfl_xor_sync(0xffffffffu, dot, 1);
+        dot += __shfl_xor_sync(pair, dot, 1);
 #pragma unroll
         for (int i = 0; i < PPL; ++i) {
             const int l = ((k0 + i) * pmagic) >> 16;
@@ -958,17 +963,47 @@ flatten_feats_kernel(const T *__restrict__ feat, const float *__restrict__ cams_
     }
 }
 
+// ------------------------------------------------------------------------------------------------
+// Reference-point refinement of the object-query decoder (decoder.py:106-118): per row
+//   ref'[c] = sigmoid(tmp[col_c] + inverse_sigmoid(ref[c])),  col = (0, 1, 4),
+// inverse_sigmoid(x) = log(max(x', eps) / max(1 - x', eps)), x' = clamp(x, 0, 1), eps = 1e-5.  Each step rounds to
+// the storage type as the reference's tensor ops do; log / exp are evaluated in double so that --use_fast_math does
+// not turn them into approximations.  ref2d (optional): the (rows, 1, 2) fp32 x, y of the result, which the next
+// layer's sampling-point prep reads.
+// ------------------------------------------------------------------------------------------------
+template <typename T>
+__global__ void __launch_bounds__(kEThreads)
+refine_points_kernel(const T *__restrict__ tmp, long long tmp_stride, const T *__restrict__ ref, T *__restrict__ out,
+                     float *__restrict__ ref2d, long long rows) {
+    const long long r = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+    if (r >= rows) return;
+    const float eps = round_to<T>(1e-5f);
+    const int cols[3] = {0, 1, 4};
+    float res[3];
+#pragma unroll
+    for (int c = 0; c < 3; ++c) {
+        const float x = fminf(fmaxf(to_f<T>(ref[r * 3 + c]), 0.f), 1.f);
+        const float x1 = fmaxf(x, eps), x2 = fmaxf(round_to<T>(__fsub_rn(1.f, x)), eps);
+        const float inv = round_to<T>((float)log((double)round_to<T>(__fdiv_rn(x1, x2))));
+        const float s = round_to<T>(__fadd_rn(to_f<T>(tmp[r * tmp_stride + cols[c]]), inv));
+        res[c] = round_to<T>(__fdiv_rn(1.f, __fadd_rn(1.f, exp_rn(-s))));
+        out[r * 3 + c] = from_f<T>(res[c]);
+    }
+    if (ref2d) reinterpret_cast<float2 *>(ref2d)[r] = make_float2(res[0], res[1]);
+}
+
 template <bool kBackward, typename TO>
 static bool launch_tsa_prep_m8(const float *raw, const float *ref2d, const float *grad_loc,
                                const float *grad_attn, const int64_t *level_hw, float *loc, float *attn,
-                               TO *d_raw, int B, int Nq, int M, int L, int P, int interleave,
+                               TO *d_raw, int B, int Nq, int M, int L, int P, int F, int interleave,
                                cudaStream_t st) {
     const int LP = L * P;
     if (!(M == 8 && L <= 16 && LP * P < 65536 && (LP == 2 || LP == 4 || LP == 8 || LP == 16 || LP == 32)))
         return false;
     const int pmagic = (65536 + P - 1) / P;
-    const unsigned grid = (unsigned)(((long long)B * Nq + kEThreads / 32 - 1) / (kEThreads / 32));
-#define BEVF_TSA_CASE(N) tsa_prep_m8<N, kBackward, TO><<<grid, kEThreads, 0, st>>>(raw, ref2d, grad_loc, grad_attn, level_hw, loc, attn, d_raw, B, Nq, L, P, pmagic, interleave)
+    const int per_block = kEThreads / (16 * F);
+    const unsigned grid = (unsigned)(((long long)B * Nq + per_block - 1) / per_block);
+#define BEVF_TSA_CASE(N) tsa_prep_m8<N, kBackward, TO><<<grid, kEThreads, 0, st>>>(raw, ref2d, grad_loc, grad_attn, level_hw, loc, attn, d_raw, B, Nq, L, P, pmagic, interleave, F)
     switch (LP / 2) {
         case 1: BEVF_TSA_CASE(1); break;
         case 2: BEVF_TSA_CASE(2); break;
@@ -1092,54 +1127,102 @@ extern "C" int bevf_sca_prep_backward_multi(const float *raw, const float *grad_
     return check_launch(who);
 }
 
-extern "C" int bevf_tsa_prep_forward(const float *raw, const float *ref2d, const int64_t *level_hw,
-                                     float *loc, float *attn, int B, int Nq, int M, int L, int P,
-                                     int interleave, void *stream) {
-    const char *who = "bevf_tsa_prep_forward";
+static int query_prep_forward(const char *who, const float *raw, const float *ref2d, const int64_t *level_hw,
+                              float *loc, float *attn, int B, int Nq, int M, int L, int P, int F, int interleave,
+                              cudaStream_t st) {
     BEVF_REQUIRE(B >= 0 && Nq >= 0 && M > 0 && L > 0 && P > 0, who, "bad dimension");
-    const long long total = (long long)B * Nq * M * 2;
+    BEVF_REQUIRE(F == 1 || F == 2, who, "frames must be 1 or 2");
+    const long long total = (long long)B * Nq * M * F;
     if (total == 0) return 0;
     BEVF_REQUIRE(raw && ref2d && level_hw && loc && attn, who, "null pointer argument");
     BEVF_REQUIRE(aligned16(raw) && aligned16(loc), who, "raw and loc must be 16-byte aligned");
     if (!launch_tsa_prep_m8<false, float>(raw, ref2d, nullptr, nullptr, level_hw, loc, attn, nullptr, B, Nq, M, L, P,
-                                   interleave, (cudaStream_t)stream)) {
+                                          F, interleave, st)) {
         if (interleave) return fail("%s: interleaved rows need num_heads == 8 and L*P in {2,4,8,16,32}", who);
-        tsa_prep_fwd<<<blocks_for(total, kEThreads), kEThreads, 0, (cudaStream_t)stream>>>(
-            raw, ref2d, level_hw, loc, attn, B, Nq, M, L, P);
+        tsa_prep_fwd<<<blocks_for(total, kEThreads), kEThreads, 0, st>>>(raw, ref2d, level_hw, loc, attn, B, Nq, M,
+                                                                         L, P, F);
     }
     return check_launch(who);
 }
 
+extern "C" int bevf_tsa_prep_forward(const float *raw, const float *ref2d, const int64_t *level_hw,
+                                     float *loc, float *attn, int B, int Nq, int M, int L, int P,
+                                     int interleave, void *stream) {
+    return query_prep_forward("bevf_tsa_prep_forward", raw, ref2d, level_hw, loc, attn, B, Nq, M, L, P, 2,
+                              interleave, (cudaStream_t)stream);
+}
+
+extern "C" int bevf_query_prep_forward(const float *raw, const float *ref2d, const int64_t *level_hw,
+                                       float *loc, float *attn, int B, int Nq, int M, int L, int P, int F,
+                                       int interleave, void *stream) {
+    return query_prep_forward("bevf_query_prep_forward", raw, ref2d, level_hw, loc, attn, B, Nq, M, L, P, F,
+                              interleave, (cudaStream_t)stream);
+}
+
 template <typename TO>
 static int tsa_prep_backward_t(const char *who, const float *raw, const float *grad_loc, const float *grad_attn,
-                               const int64_t *level_hw, TO *d_raw, int B, int Nq, int M, int L, int P,
+                               const int64_t *level_hw, TO *d_raw, int B, int Nq, int M, int L, int P, int F,
                                int interleave, cudaStream_t st) {
-    const long long total = (long long)B * Nq * M * 2;
+    const long long total = (long long)B * Nq * M * F;
     if (!launch_tsa_prep_m8<true, TO>(raw, nullptr, grad_loc, grad_attn, level_hw, nullptr, nullptr, d_raw, B, Nq, M,
-                                      L, P, interleave, st)) {
+                                      L, P, F, interleave, st)) {
         if (interleave) return fail("%s: interleaved rows need num_heads == 8 and L*P in {2,4,8,16,32}", who);
         tsa_prep_bwd<TO><<<blocks_for(total, kEThreads), kEThreads, 0, st>>>(
-            raw, grad_loc, grad_attn, level_hw, d_raw, B, Nq, M, L, P);
+            raw, grad_loc, grad_attn, level_hw, d_raw, B, Nq, M, L, P, F);
     }
     return check_launch(who);
+}
+
+static int query_prep_backward(const char *who, const float *raw, const float *grad_loc, const float *grad_attn,
+                               const int64_t *level_hw, void *d_raw, int out_dtype, int B, int Nq, int M, int L,
+                               int P, int F, int interleave, cudaStream_t st) {
+    BEVF_REQUIRE(B >= 0 && Nq >= 0 && M > 0 && L > 0 && P > 0, who, "bad dimension");
+    BEVF_REQUIRE(F == 1 || F == 2, who, "frames must be 1 or 2");
+    BEVF_REQUIRE(out_dtype == BEVF_DTYPE_F32 || out_dtype == BEVF_DTYPE_BF16 || out_dtype == BEVF_DTYPE_F16, who, "unsupported dtype code");
+    if ((long long)B * Nq * M * F == 0) return 0;
+    BEVF_REQUIRE(raw && grad_loc && grad_attn && level_hw && d_raw, who, "null pointer argument");
+    BEVF_REQUIRE(aligned16(raw) && aligned16(d_raw), who, "raw and d_raw must be 16-byte aligned");
+    if (out_dtype == BEVF_DTYPE_BF16)
+        return tsa_prep_backward_t<bf16>(who, raw, grad_loc, grad_attn, level_hw, (bf16 *)d_raw, B, Nq, M, L, P, F, interleave, st);
+    if (out_dtype == BEVF_DTYPE_F16)
+        return tsa_prep_backward_t<__half>(who, raw, grad_loc, grad_attn, level_hw, (__half *)d_raw, B, Nq, M, L, P, F, interleave, st);
+    return tsa_prep_backward_t<float>(who, raw, grad_loc, grad_attn, level_hw, (float *)d_raw, B, Nq, M, L, P, F, interleave, st);
 }
 
 extern "C" int bevf_tsa_prep_backward(const float *raw, const float *grad_loc,
                                       const float *grad_attn, const int64_t *level_hw, void *d_raw,
                                       int out_dtype, int B, int Nq, int M, int L, int P, int interleave,
                                       void *stream) {
-    const char *who = "bevf_tsa_prep_backward";
-    BEVF_REQUIRE(B >= 0 && Nq >= 0 && M > 0 && L > 0 && P > 0, who, "bad dimension");
-    BEVF_REQUIRE(out_dtype == BEVF_DTYPE_F32 || out_dtype == BEVF_DTYPE_BF16 || out_dtype == BEVF_DTYPE_F16, who, "unsupported dtype code");
-    if ((long long)B * Nq * M * 2 == 0) return 0;
-    BEVF_REQUIRE(raw && grad_loc && grad_attn && level_hw && d_raw, who, "null pointer argument");
-    BEVF_REQUIRE(aligned16(raw) && aligned16(d_raw), who, "raw and d_raw must be 16-byte aligned");
+    return query_prep_backward("bevf_tsa_prep_backward", raw, grad_loc, grad_attn, level_hw, d_raw, out_dtype, B, Nq,
+                               M, L, P, 2, interleave, (cudaStream_t)stream);
+}
+
+extern "C" int bevf_query_prep_backward(const float *raw, const float *grad_loc, const float *grad_attn,
+                                        const int64_t *level_hw, void *d_raw, int out_dtype, int B, int Nq, int M,
+                                        int L, int P, int F, int interleave, void *stream) {
+    return query_prep_backward("bevf_query_prep_backward", raw, grad_loc, grad_attn, level_hw, d_raw, out_dtype, B,
+                               Nq, M, L, P, F, interleave, (cudaStream_t)stream);
+}
+
+template <typename T>
+static int refine_points_t(const void *tmp, long long tmp_stride, const void *ref, void *out, float *ref2d,
+                           long long rows, cudaStream_t st) {
+    refine_points_kernel<T><<<blocks_for(rows, kEThreads), kEThreads, 0, st>>>(
+        (const T *)tmp, tmp_stride, (const T *)ref, (T *)out, ref2d, rows);
+    return check_launch("bevf_refine_points");
+}
+
+extern "C" int bevf_refine_points(const void *tmp, int64_t tmp_row_stride, const void *ref, void *out, float *ref2d,
+                                  int dtype, int64_t rows, void *stream) {
+    const char *who = "bevf_refine_points";
+    BEVF_REQUIRE(rows >= 0 && tmp_row_stride >= 5, who, "bad dimension (the regression row needs 5 columns)");
+    BEVF_REQUIRE(dtype == BEVF_DTYPE_F32 || dtype == BEVF_DTYPE_BF16 || dtype == BEVF_DTYPE_F16, who, "unsupported dtype code");
+    if (rows == 0) return 0;
+    BEVF_REQUIRE(tmp && ref && out, who, "null pointer argument");
     cudaStream_t st = (cudaStream_t)stream;
-    if (out_dtype == BEVF_DTYPE_BF16)
-        return tsa_prep_backward_t<bf16>(who, raw, grad_loc, grad_attn, level_hw, (bf16 *)d_raw, B, Nq, M, L, P, interleave, st);
-    if (out_dtype == BEVF_DTYPE_F16)
-        return tsa_prep_backward_t<__half>(who, raw, grad_loc, grad_attn, level_hw, (__half *)d_raw, B, Nq, M, L, P, interleave, st);
-    return tsa_prep_backward_t<float>(who, raw, grad_loc, grad_attn, level_hw, (float *)d_raw, B, Nq, M, L, P, interleave, st);
+    if (dtype == BEVF_DTYPE_BF16) return refine_points_t<bf16>(tmp, tmp_row_stride, ref, out, ref2d, rows, st);
+    if (dtype == BEVF_DTYPE_F16) return refine_points_t<__half>(tmp, tmp_row_stride, ref, out, ref2d, rows, st);
+    return refine_points_t<float>(tmp, tmp_row_stride, ref, out, ref2d, rows, st);
 }
 
 template <typename T, typename TP>

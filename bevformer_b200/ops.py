@@ -851,6 +851,78 @@ class TsaPrep(Function):
         return (d_raw,) + (None,) * 8
 
 
+def query_prep_forward(raw, ref2d, level_hw, B, Nq, M, L, P, F, interleave=False):
+    """(loc, attn) of the query-side sampling points for F frames (bevf_query_prep_forward); F = 2 is TSA's
+    tsa_prep_forward, F = 1 the decoder's CustomMSDeformableAttention."""
+    _need_cuda(raw, "raw")
+    shape = (B * Nq * F, M, L, P) if interleave else (B * F, Nq, M, L, P)
+    loc = torch.empty(shape + (2,), device=raw.device, dtype=torch.float32)
+    attn = torch.empty(shape, device=raw.device, dtype=torch.float32)
+    lib = _lib.load()
+    with torch.cuda.device(raw.device):
+        st = lib.bevf_query_prep_forward(raw.data_ptr(), ref2d.data_ptr(), level_hw.data_ptr(), loc.data_ptr(),
+                                         attn.data_ptr(), B, Nq, M, L, P, F, int(interleave), _stream_ptr(raw))
+    _lib.check(st, lib)
+    return loc, attn
+
+
+def query_prep_backward(raw, grad_loc, grad_attn, level_hw, B, Nq, M, L, P, F, interleave=0,
+                        out_dtype=torch.float32):
+    d_raw = torch.empty(raw.shape, device=raw.device, dtype=out_dtype)
+    lib = _lib.load()
+    with torch.cuda.device(raw.device):
+        st = lib.bevf_query_prep_backward(raw.data_ptr(), grad_loc.contiguous().data_ptr(),
+                                          grad_attn.contiguous().data_ptr(), level_hw.data_ptr(), d_raw.data_ptr(),
+                                          _DT[out_dtype], B, Nq, M, L, P, F, int(interleave), _stream_ptr(raw))
+    _lib.check(st, lib)
+    return d_raw
+
+
+class QueryPrep(Function):
+    """query_prep_forward as an autograd node on an fp32 ``raw`` (the 16-bit path fuses it with the head GEMM,
+    plugin.linear)."""
+
+    @staticmethod
+    def forward(ctx, raw, ref2d, level_hw, B, Nq, M, L, P, F):
+        loc, attn = query_prep_forward(raw, ref2d, level_hw, B, Nq, M, L, P, F)
+        ctx.save_for_backward(raw, level_hw)
+        ctx.dims = (B, Nq, M, L, P, F)
+        return loc, attn
+
+    @staticmethod
+    @once_differentiable
+    def backward(ctx, grad_loc, grad_attn):
+        raw, level_hw = ctx.saved_tensors
+        d_raw = query_prep_backward(raw, grad_loc, grad_attn, level_hw, *ctx.dims)
+        return (d_raw,) + (None,) * 8
+
+
+def refine_points(tmp, ref, with_ref2d=True):
+    """DetectionTransformerDecoder's reference-point refinement (decoder.py:106-118) in one kernel:
+    sigmoid(tmp[..., (0, 1, 4)] + inverse_sigmoid(ref)) for ref (..., 3) and the regression output tmp (..., >= 5),
+    both in one dtype; tmp is read in place (its last dim must be contiguous).  Returns (new ref (..., 3) in that
+    dtype, its x, y as a contiguous (..., 1, 2) fp32 tensor -- the next layer's prep input -- or None).  No autograd:
+    the result is detached, as in the reference."""
+    _need_cuda(ref, "ref")
+    if tmp.dtype != ref.dtype:
+        raise RuntimeError(f"refine_points: tmp ({tmp.dtype}) and ref ({ref.dtype}) must share one dtype")
+    if ref.shape[-1] != 3 or tmp.shape[:-1] != ref.shape[:-1] or tmp.shape[-1] < 5:
+        raise RuntimeError(f"refine_points: shapes {tuple(tmp.shape)} / {tuple(ref.shape)}: need (..., >=5) / (..., 3)")
+    rows = ref.numel() // 3
+    tmp2 = tmp.reshape(rows, tmp.shape[-1])
+    if tmp2.stride(1) != 1:
+        tmp2 = tmp2.contiguous()
+    ref = ref.contiguous()
+    out = torch.empty_like(ref)
+    ref2d = torch.empty(ref.shape[:-1] + (1, 2), device=ref.device, dtype=torch.float32) if with_ref2d else None
+    lib = _lib.load()
+    with torch.cuda.device(ref.device):
+        st = lib.bevf_refine_points(tmp2.data_ptr(), tmp2.stride(0), ref.data_ptr(), out.data_ptr(), _ptr(ref2d),
+                                    _DT[ref.dtype], rows, _stream_ptr(ref))
+    _lib.check(st, lib)
+    return out, ref2d
+
+
 def _ptr(t):
     return 0 if t is None else t.data_ptr()
 

@@ -11,8 +11,10 @@ projects/configs/bevformer/*.py builds unchanged (SURVEY.md §8 f2).
 
 The shapes here are small (900 queries, one 200x200 level, 4 points): the value projection over the
 40 000 BEV cells is the only part with real work -- it and the other projections run on the wgmma
-GEMM, the gather on the sampler kernel; the few-KB softmax / offset arithmetic in between stays in
-tensor ops.
+GEMM, the gather on the sampler kernel.  What sits between the library calls is fused too, because at these
+sizes a decoder layer is bound by launches: the sampling-point prep runs on the TSA prep kernels with one
+frame (``bevf_query_prep_*``), the reference-point refinement is one kernel (``bevf_refine_points``) and the
+object-query self-attention runs on the attention kernel.
 """
 from __future__ import annotations
 
@@ -23,7 +25,7 @@ import copy
 import warnings
 
 from .. import ops, precision
-from .linear import linear, linear_fp32_out
+from .linear import linear, linear_fp32_out, query_sampling_head
 from .registry import (ATTENTION, HAVE_MMCV, TRANSFORMER_LAYER, TRANSFORMER_LAYER_SEQUENCE, _register,
                        build_transformer_layer)
 from .temporal_self_attention import _check_head_dim, ring_offsets_
@@ -93,6 +95,21 @@ class CustomMSDeformableAttention(nn.Module):
         v = v.reshape(bs, nv, m, -1)
         w = torch.cat([self.sampling_offsets.weight, self.attention_weights.weight], 0)
         b = torch.cat([self.sampling_offsets.bias, self.attention_weights.bias], 0)
+        if reference_points.shape[-1] == 2 and query.is_cuda:
+            # the offsets|logits head and the softmax / offset / (W, H) + reference point prep (:300-330) as one
+            # node: the TSA prep kernels with one frame
+            ref = reference_points.reshape(bs, nq, l, 2).float().contiguous()
+            loc, att = query_sampling_head(query, w, b, ref, ss.contiguous(), bs, nq, m, l, p)
+            if reference_points.requires_grad and torch.is_grad_enabled():
+                # the prep reads the reference points as a constant; their gradient (grad_loc summed over heads
+                # and points, what the reference's broadcast add gives them) flows through this zero-valued term
+                d = reference_points.reshape(bs, nq, l, 2).float()
+                loc = loc + (d - d.detach())[:, :, None, :, None, :]
+            out = ops.MultiScaleDeformableAttnFunction_fp32.apply(v, ss, lsi, loc, att, self.im2col_step)
+            out = linear(out.to(query.dtype), self.output_proj.weight, self.output_proj.bias)
+            if not self.batch_first:
+                out = out.permute(1, 0, 2)
+            return self.dropout(out) + identity
         raw = linear_fp32_out(query, w, b)                                   # (bs, nq, m*l*p*3) fp32
         n_off = m * l * p * 2
         off = raw[..., :n_off].reshape(bs, nq, m, l, p, 2)
@@ -123,10 +140,42 @@ def inverse_sigmoid(x, eps=1e-5):
     return torch.log(x.clamp(min=eps) / (1 - x).clamp(min=eps))
 
 
-class MultiheadAttention(nn.Module):
+class _KernelAttention(nn.Module):
+    """The attention-kernel route shared by mmcv's ``MultiheadAttention`` wrapper and ``GroupMultiheadAttention``
+    (both keep their ``nn.MultiheadAttention`` as ``self.attn``): 16-bit CUDA inputs with head_dim 32 and no masks
+    run the in-projection on the wgmma GEMM (one GEMM over the [W_q; W_k] rows when query and key are the same
+    tensor), ``ops.GroupAttention`` (Philox dropout in training) and the out-projection on the GEMM."""
+
+    def _kernel_ok(self, query, key, attn_mask, key_padding_mask, groups):
+        a = self.attn
+        return (query.is_cuda and query.dtype in ops.TC_DTYPES and key.dtype == query.dtype
+                and attn_mask is None and key_padding_mask is None
+                and self.embed_dims == self.num_heads * 32 and a._qkv_same_embed_dim and a.bias_k is None
+                and not a.add_zero_attn and not a.batch_first and (groups == 1 or key.shape[0] == query.shape[0]))
+
+    def _forward_kernel(self, qin, kin, value, shared, groups):
+        a, C = self.attn, self.embed_dims
+        w, b = a.in_proj_weight, a.in_proj_bias
+        bq = (lambda lo, hi: None) if b is None else (lambda lo, hi: b[lo:hi])
+        v = linear(value, w[2 * C:], bq(2 * C, 3 * C))
+        drop = a.dropout if self.training else 0.0
+        scale = float(C // self.num_heads) ** -0.5
+        if shared:
+            qk = linear(qin, w[:2 * C], bq(0, 2 * C))
+            out = ops.GroupAttention.apply(qk, None, v, self.num_heads, groups, scale, drop)
+        else:
+            q = linear(qin, w[:C], bq(0, C))
+            k = linear(kin, w[C:2 * C], bq(C, 2 * C))
+            out = ops.GroupAttention.apply(q, k, v, self.num_heads, groups, scale, drop)
+        return linear(out, a.out_proj.weight, a.out_proj.bias)
+
+
+class MultiheadAttention(_KernelAttention):
     """mmcv's wrapper around nn.MultiheadAttention (mmcv/cnn/bricks/transformer.py, 1.4.0): positional
     encodings added to query / key, optional batch-first layout, ``identity + dropout_layer(proj_drop(attn))``.
-    The object-query self-attention of the decoder (900 queries): a library attention call, not a hot path."""
+    The object-query self-attention of the decoder (900 queries): on the attention kernel with ``groups = 1``
+    (_KernelAttention) for 16-bit CUDA inputs, head_dim 32 and no masks; fp32 and masked calls keep
+    ``nn.MultiheadAttention``."""
 
     def __init__(self, embed_dims, num_heads, attn_drop=0.0, proj_drop=0.0,
                  dropout_layer=dict(type="Dropout", drop_prob=0.0), init_cfg=None, batch_first=False, **kwargs):
@@ -152,14 +201,20 @@ class MultiheadAttention(nn.Module):
             identity = query
         if key_pos is None and query_pos is not None and query_pos.shape == key.shape:
             key_pos = query_pos
+        shared = key is query and key_pos is query_pos       # self-attention: Q and K projected by one GEMM
         if query_pos is not None:
             query = query + query_pos
-        if key_pos is not None:
+        if shared:
+            key = query
+        elif key_pos is not None:
             key = key + key_pos
         if self.batch_first:
             query, key, value = query.transpose(0, 1), key.transpose(0, 1), value.transpose(0, 1)
-        out = self.attn(query=query, key=key, value=value, attn_mask=attn_mask,
-                        key_padding_mask=key_padding_mask)[0]
+        if self._kernel_ok(query, key, attn_mask, key_padding_mask, 1):
+            out = self._forward_kernel(query, key, value, shared, 1)
+        else:
+            out = self.attn(query=query, key=key, value=value, attn_mask=attn_mask,
+                            key_padding_mask=key_padding_mask)[0]
         if self.batch_first:
             out = out.transpose(0, 1)
         return identity + self.dropout_layer(self.proj_drop(out))
@@ -168,7 +223,7 @@ class MultiheadAttention(nn.Module):
 _GROUP_DROPOUT_DEFAULT = dict(type="Dropout", drop_prob=0.)
 
 
-class GroupMultiheadAttention(nn.Module):
+class GroupMultiheadAttention(_KernelAttention):
     """Group DETR's decoder self-attention (group_attention.py:18-162): mmcv's MultiheadAttention wrapper whose
     ``num_query`` queries split, in training only, into ``group`` equal slices that attend only within their own
     slice.  The BEVFormerV2 configs train 11 groups of 900 queries (9900) and evaluate one group.
@@ -202,13 +257,6 @@ class GroupMultiheadAttention(nn.Module):
             raise NotImplementedError(f"GroupMultiheadAttention: dropout_layer type {dropout_layer['type']!r} is not "
                                       "supported (only 'Dropout')")
         self.dropout_layer = nn.Dropout(dropout_layer.get("drop_prob", 0.0)) if dropout_layer else nn.Identity()
-
-    def _kernel_ok(self, query, key, attn_mask, key_padding_mask, groups):
-        a = self.attn
-        return (query.is_cuda and query.dtype in ops.TC_DTYPES and key.dtype == query.dtype
-                and attn_mask is None and key_padding_mask is None
-                and self.embed_dims == self.num_heads * 32 and a._qkv_same_embed_dim and a.bias_k is None
-                and not a.add_zero_attn and not a.batch_first and (groups == 1 or key.shape[0] == query.shape[0]))
 
     @precision.entry("query", "key", "value", "identity", "query_pos", "key_pos")
     def forward(self, query, key=None, value=None, identity=None, query_pos=None, key_pos=None,
@@ -247,22 +295,6 @@ class GroupMultiheadAttention(nn.Module):
             out = out.transpose(0, 1)
         return identity + self.dropout_layer(self.proj_drop(out))
 
-    def _forward_kernel(self, qin, kin, value, shared, groups):
-        a, C = self.attn, self.embed_dims
-        w, b = a.in_proj_weight, a.in_proj_bias
-        bq = (lambda lo, hi: None) if b is None else (lambda lo, hi: b[lo:hi])
-        v = linear(value, w[2 * C:], bq(2 * C, 3 * C))
-        drop = a.dropout if self.training else 0.0
-        scale = float(C // self.num_heads) ** -0.5
-        if shared:
-            qk = linear(qin, w[:2 * C], bq(0, 2 * C))
-            out = ops.GroupAttention.apply(qk, None, v, self.num_heads, groups, scale, drop)
-        else:
-            q = linear(qin, w[:C], bq(0, C))
-            k = linear(kin, w[C:2 * C], bq(C, 2 * C))
-            out = ops.GroupAttention.apply(q, k, v, self.num_heads, groups, scale, drop)
-        return linear(out, a.out_proj.weight, a.out_proj.bias)
-
     def _forward_torch(self, query, key, value, attn_mask, key_padding_mask, nq, bs):
         """The reference's arithmetic: groups moved to the batch axis around nn.MultiheadAttention."""
         if self.training:
@@ -294,6 +326,17 @@ def _decoder_layer_cls():
     return DetrTransformerDecoderLayer
 
 
+def _run_branch(branch, x):
+    """A head branch (the caller's module) on a decoder output.  Inside an entry point autocast is off; a 16-bit
+    output meeting an fp32 branch then runs the branch under autocast in that dtype, as the caller's autocast
+    would have."""
+    p = next(branch.parameters(), None)
+    if x.is_cuda and x.dtype in (torch.bfloat16, torch.float16) and p is not None and p.dtype != x.dtype:
+        with torch.autocast(device_type="cuda", dtype=x.dtype):
+            return branch(x)
+    return branch(x)
+
+
 class DetectionTransformerDecoder(nn.Module):
     """The DETR3D-style decoder (decoder.py:52-129): ``num_layers`` decoder layers; after each, the
     layer's regression branch refines the (x, y, z) reference points in inverse-sigmoid space and the
@@ -322,18 +365,23 @@ class DetectionTransformerDecoder(nn.Module):
         (stack of layer outputs, stack of reference points) with return_intermediate, else the last pair."""
         output = query
         intermediate, intermediate_reference_points = [], []
+        ref2d = None            # the refinement kernel's fp32 (bs, nq, 1, 2) copy of reference_points[..., :2]
         for lid, layer in enumerate(self.layers):
-            reference_points_input = reference_points[..., :2].unsqueeze(2)       # (bs, nq, num_levels=1, 2)
+            reference_points_input = reference_points[..., :2].unsqueeze(2) if ref2d is None else ref2d
             output = layer(output, *args, reference_points=reference_points_input,
                            key_padding_mask=key_padding_mask, **kwargs)
             output = output.permute(1, 0, 2)
             if reg_branches is not None:
-                tmp = reg_branches[lid](output)
+                tmp = _run_branch(reg_branches[lid], output)
                 assert reference_points.shape[-1] == 3
-                new_reference_points = torch.zeros_like(reference_points)
-                new_reference_points[..., :2] = tmp[..., :2] + inverse_sigmoid(reference_points[..., :2])
-                new_reference_points[..., 2:3] = tmp[..., 4:5] + inverse_sigmoid(reference_points[..., 2:3])
-                reference_points = new_reference_points.sigmoid().detach()
+                if tmp.is_cuda and tmp.dtype == reference_points.dtype:
+                    # one kernel for the zeros_like / two inverse_sigmoid / slice assignments / sigmoid below
+                    reference_points, ref2d = ops.refine_points(tmp.detach(), reference_points.detach())
+                else:
+                    new_reference_points = torch.zeros_like(reference_points)
+                    new_reference_points[..., :2] = tmp[..., :2] + inverse_sigmoid(reference_points[..., :2])
+                    new_reference_points[..., 2:3] = tmp[..., 4:5] + inverse_sigmoid(reference_points[..., 2:3])
+                    reference_points = new_reference_points.sigmoid().detach()
             output = output.permute(1, 0, 2)
             if self.return_intermediate:
                 intermediate.append(output)

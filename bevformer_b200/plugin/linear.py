@@ -312,6 +312,9 @@ class _HeadTC(Function):
         if kind == "sca":
             ref_cam, pair_q, pair_cam, pair_of, ss, bs, nq, m, l, p = prep_args
             loc, attn = ops.sca_prep_forward(raw, ref_cam, pair_q, pair_cam, ss, bs, nq, m, l, p)
+        elif kind == "query":
+            ref, ss, bs, nq, m, l, p = prep_args
+            loc, attn = ops.query_prep_forward(raw, ref, ss, bs, nq, m, l, p, 1)
         else:
             ref, ss, bs, nq, m, l, p, interleave = prep_args
             loc, attn = ops.tsa_prep_forward(raw, ref, ss, bs, nq, m, l, p, interleave)
@@ -330,6 +333,9 @@ class _HeadTC(Function):
             _ref_cam, pair_q, _pair_cam, pair_of, ss, bs, nq, m, l, p = ctx.prep_args
             d_raw = ops.sca_prep_backward(raw, grad_loc, grad_attn, pair_of, ss, bs, nq,
                                           pair_q.numel(), m, l, p, out_dtype=w.dtype)
+        elif ctx.kind == "query":
+            _ref, ss, bs, nq, m, l, p = ctx.prep_args
+            d_raw = ops.query_prep_backward(raw, grad_loc, grad_attn, ss, bs, nq, m, l, p, 1, out_dtype=w.dtype)
         else:
             _ref, ss, bs, nq, m, l, p, interleave = ctx.prep_args
             d_raw = ops.tsa_prep_backward(raw, grad_loc, grad_attn, ss, bs, nq, m, l, p, interleave,
@@ -415,6 +421,15 @@ def sca_head_sampler(x, weight, bias, value, fuse):
     """Sampler output (bs*pairs, C) of SpatialCrossAttention straight from the query: the offsets|logits head and the
     row-list sampler with the sampling-point prep fused in (_ScaHeadSamplerTC; the caller checks that it applies)."""
     return _ScaHeadSamplerTC.apply(x, weight, bias, value, fuse)
+
+
+def query_sampling_head(x, weight, bias, ref, ss, bs, nq, m, l, p):
+    """(loc, attn) of the decoder's CustomMSDeformableAttention for 2-d reference points (decoder.py:300-330): the
+    TSA prep with one frame.  16-bit x: one node with the head GEMM, d_raw in 16 bits; fp32: GEMM + QueryPrep."""
+    if _use_tc(x, weight):
+        return _HeadTC.apply(x, weight, bias, "query", (ref, ss, bs, nq, m, l, p))
+    raw = linear_fp32_out(x, weight, bias).reshape(bs * nq, -1)
+    return ops.QueryPrep.apply(raw, ref, ss, bs, nq, m, l, p, 1)
 
 
 def tsa_sampling_head(x, weight, bias, ref, ss, bs, nq, m, l, p, interleave=False):

@@ -7,7 +7,9 @@ training step at base) and ``BEVFormer.forward_test`` (:236-269, state initialis
 ``prev_frame_info`` from frame to frame.  Both reach the encoder through
 ``pts_bbox_head(..., only_bev=True)`` -> ``transformer.get_bev_features`` (dense_heads/bevformer_head.py);
 here they call ``PerceptionTransformer.get_bev_features`` of this package directly: the detector and head
-classes themselves (backbone, FPN, query embeddings, losses) are outside the hot path.
+classes themselves (backbone, FPN, query embeddings, losses) are outside the hot path.  Given the head's object
+query embedding (and regression branches), ``BEVStream`` runs the whole transformer per frame instead --
+``PerceptionTransformer.forward``, encoder and decoder, as forward_test does through the head (:263-268).
 
 Both take the per-frame CAN-bus vectors and camera matrices either from the metas (host path: numpy + torchvision
 once per frame, as the reference) or as CUDA tensors ``can_bus=`` / ``lidar2img=`` (device path: two kernels, no
@@ -82,6 +84,11 @@ class BEVStream:
                       ``bevf_ego_motion`` reads and advances; the step never synchronises with the host;
       * captured      after ``capture(...)``: the device path recorded as two CUDA graphs (first frame of a scene,
                       continuation); ``step`` replays the one the scene token selects.
+    With ``object_query_embed`` (num_query, 2C) given -- to ``step``, or to ``capture`` for the captured mode -- a
+    frame is the whole transformer (``transformer.forward``: encoder, then the object-query decoder with
+    ``reg_branches`` / ``cls_branches``) and returns its 4-tuple (bev_embed (Nq, bs, C), inter_states,
+    init_reference_out, inter_references_out); bev_embed becomes the next frame's prev_bev.  Without it a frame is
+    ``get_bev_features`` and returns the BEV alone.
     ``prev_frame_info["scene_token"]`` and ``["prev_bev"]`` are shared by the three; do not mix the host path with
     the other two inside one scene (each keeps its own previous position / angle)."""
 
@@ -100,7 +107,8 @@ class BEVStream:
 
     @torch.no_grad()
     def step(self, mlvl_feats: Optional[List[torch.Tensor]], img_metas: List[dict], bev_queries=None, bev_h: int = None,
-             bev_w: int = None, bev_pos=None, grid_length=(0.512, 0.512), can_bus=None, lidar2img=None) -> torch.Tensor:
+             bev_w: int = None, bev_pos=None, grid_length=(0.512, 0.512), can_bus=None, lidar2img=None,
+             object_query_embed=None, reg_branches=None, cls_branches=None):
         """One frame: mlvl_feats per level (bs, num_cams, C, h, w), img_metas one dict per sample with
         ABSOLUTE ``can_bus`` and a ``scene_token``.  Returns this frame's BEV (bs, Nq, C), which also becomes
         the next frame's ``prev_bev``.  The caller's metas are not modified (the reference edits them in
@@ -110,9 +118,13 @@ class BEVStream:
         read; ``scene_token`` and ``img_shape`` are).  Captured mode: only ``img_metas[0]["scene_token"]`` is read;
         tensors passed for ``mlvl_feats`` / ``can_bus`` / ``lidar2img`` are copied into the static buffers, ``None``
         means the caller has filled ``self.static`` itself.  The BEV returned in captured mode is the static
-        output buffer: it is OVERWRITTEN by the next ``step`` (clone it to keep it)."""
+        output buffer: it is OVERWRITTEN by the next ``step`` (clone it to keep it).
+
+        ``object_query_embed`` / ``reg_branches`` / ``cls_branches``: run the whole transformer and return its 4-tuple
+        (in captured mode, what ``capture`` was given decides, and these are ignored)."""
         if self._graphs is not None:
             return self._step_captured(mlvl_feats, img_metas, can_bus, lidar2img)
+        head = None if object_query_embed is None else (object_query_embed, reg_branches, cls_branches)
         info = self.prev_frame_info
         if img_metas[0].get("scene_token") != info["scene_token"]:
             info["prev_bev"] = None                                  # :243-245
@@ -120,10 +132,10 @@ class BEVStream:
         if not self.video_test_mode:
             info["prev_bev"] = None                                  # :249-251
         if _on_device(can_bus):
-            bev = self._frame(mlvl_feats, img_metas, bev_queries, bev_h, bev_w, bev_pos, grid_length, can_bus,
-                              lidar2img, info["prev_bev"])
-            info["prev_bev"] = bev
-            return bev
+            res = self._frame(mlvl_feats, img_metas, bev_queries, bev_h, bev_w, bev_pos, grid_length, can_bus,
+                              lidar2img, info["prev_bev"], head)
+            info["prev_bev"] = res if head is None else res[0]
+            return res
         metas = [dict(m) for m in img_metas]
         can_bus = np.array(metas[0]["can_bus"], dtype=np.float64, copy=True)
         tmp_pos, tmp_angle = can_bus[:3].copy(), copy.deepcopy(can_bus[-1])      # :254-255
@@ -137,17 +149,26 @@ class BEVStream:
         was_training = self.transformer.training
         self.transformer.eval()
         try:
-            bev = self.transformer.get_bev_features(mlvl_feats, bev_queries, bev_h, bev_w,
-                                                    grid_length=list(grid_length), bev_pos=bev_pos,
-                                                    prev_bev=info["prev_bev"], img_metas=metas)
+            res = self._run(head, mlvl_feats, bev_queries, bev_h, bev_w, grid_length=list(grid_length),
+                            bev_pos=bev_pos, prev_bev=info["prev_bev"], img_metas=metas)
         finally:
             self.transformer.train(was_training)
+        bev = res if head is None else res[0]
         info["prev_pos"], info["prev_angle"], info["prev_bev"] = tmp_pos, tmp_angle, bev    # :266-268
-        return bev
+        return res
+
+    def _run(self, head, mlvl_feats, bev_queries, bev_h, bev_w, **kwargs):
+        """get_bev_features, or with ``head`` = (object_query_embed, reg_branches, cls_branches) the whole
+        transformer."""
+        if head is None:
+            return self.transformer.get_bev_features(mlvl_feats, bev_queries, bev_h, bev_w, **kwargs)
+        oq, reg, cls = head
+        return self.transformer(mlvl_feats, bev_queries, oq, bev_h, bev_w, reg_branches=reg, cls_branches=cls,
+                                **kwargs)
 
     # ---- device path --------------------------------------------------------------------------------------------
     def _frame(self, mlvl_feats, img_metas, bev_queries, bev_h, bev_w, bev_pos, grid_length, can_bus, lidar2img,
-               prev_bev):
+               prev_bev, head=None):
         """One device-path frame; the delta step of forward_test (:254-268) happens inside bevf_ego_motion."""
         if self.ego_state is None:
             self.ego_state = ops.ego_state(can_bus.device)
@@ -155,17 +176,18 @@ class BEVStream:
         was_training = self.transformer.training
         self.transformer.eval()
         try:
-            return self.transformer.get_bev_features(
-                mlvl_feats, bev_queries, bev_h, bev_w, grid_length=list(grid_length), bev_pos=bev_pos,
-                prev_bev=prev_bev, img_metas=img_metas, can_bus=can_bus, ego_state=self.ego_state,
-                ego_mode=ops.EGO_NEW_SCENE if prev_bev is None else ops.EGO_CONTINUE, **extra)
+            return self._run(head, mlvl_feats, bev_queries, bev_h, bev_w, grid_length=list(grid_length),
+                             bev_pos=bev_pos, prev_bev=prev_bev, img_metas=img_metas, can_bus=can_bus,
+                             ego_state=self.ego_state,
+                             ego_mode=ops.EGO_NEW_SCENE if prev_bev is None else ops.EGO_CONTINUE, **extra)
         finally:
             self.transformer.train(was_training)
 
     # ---- captured mode ------------------------------------------------------------------------------------------
     @torch.no_grad()
     def capture(self, mlvl_feats: List[torch.Tensor], img_metas: List[dict], bev_queries, bev_h: int, bev_w: int,
-                bev_pos, grid_length=(0.512, 0.512), *, can_bus, lidar2img) -> dict:
+                bev_pos, grid_length=(0.512, 0.512), *, can_bus, lidar2img, object_query_embed=None,
+                reg_branches=None, cls_branches=None) -> dict:
         """Record the device path for these shapes as two CUDA graphs -- first frame of a scene (no history: the
         temporal self-attention stacks the query with itself) and continuation (prev_bev = the previous output,
         rotated) -- over static input buffers, returned (and kept as ``self.static``): ``{"feats": [per level],
@@ -175,7 +197,10 @@ class BEVStream:
         encoder's pair list from the rig given here, + 15 %, which synchronises once); the stream is reset
         afterwards.  A replay cannot report a pair-list overflow (``BEVFormerEncoder.check_plan`` sees eager forwards
         only): before replaying a rig that may put more pairs in view than the captured one, run one eager
-        device-path frame with it and ``encoder.check_plan()``, and capture again if that raises."""
+        device-path frame with it and ``encoder.check_plan()``, and capture again if that raises.
+
+        With ``object_query_embed`` the graphs record the whole transformer (encoder and decoder; the embedding and
+        the branches are read in place by every replay) and ``step`` returns the static 4-tuple of output buffers."""
         if not (_on_device(can_bus) and _on_device(lidar2img)):
             raise RuntimeError("BEVStream.capture: can_bus and lidar2img must be CUDA tensors (the device path)")
         self._graphs = None
@@ -183,7 +208,8 @@ class BEVStream:
                            can_bus=can_bus.detach().to(torch.float64).reshape(-1, 18).clone(),
                            lidar2img=lidar2img.detach().to(torch.float32).clone())
         self._cap = dict(img_metas=[dict(img_shape=img_metas[0]["img_shape"]) for _ in img_metas],
-                         bev_queries=bev_queries, bev_h=bev_h, bev_w=bev_w, bev_pos=bev_pos, grid_length=grid_length)
+                         bev_queries=bev_queries, bev_h=bev_h, bev_w=bev_w, bev_pos=bev_pos, grid_length=grid_length,
+                         head=None if object_query_embed is None else (object_query_embed, reg_branches, cls_branches))
         self._record()
         return self.static
 
@@ -192,24 +218,26 @@ class BEVStream:
         c, st = self._cap, self.static
         dev = st["can_bus"].device
 
-        def frame(prev):
-            return self._frame(st["feats"], c["img_metas"], c["bev_queries"], c["bev_h"], c["bev_w"], c["bev_pos"],
-                               c["grid_length"], st["can_bus"], st["lidar2img"], prev)
+        def frame(prev):                                   # the frame's outputs as a tuple, bev first
+            res = self._frame(st["feats"], c["img_metas"], c["bev_queries"], c["bev_h"], c["bev_w"], c["bev_pos"],
+                              c["grid_length"], st["can_bus"], st["lidar2img"], prev, c["head"])
+            return (res,) if c["head"] is None else tuple(res)
 
         cur = torch.cuda.current_stream(dev)
         side = torch.cuda.Stream(dev)
         side.wait_stream(cur)
         with torch.cuda.stream(side):                      # eager warm-up of both kinds of frame
-            out = frame(None).clone()
-            frame(out)
+            outs = tuple(t.clone() for t in frame(None))
+            frame(outs[0])
         cur.wait_stream(side)
         graphs, pool = {}, None
         for kind in ("first", "cont"):
             g = torch.cuda.CUDAGraph()
             with torch.cuda.graph(g, pool=pool):
-                out.copy_(frame(None if kind == "first" else out))
+                for o, r in zip(outs, frame(None if kind == "first" else outs[0])):
+                    o.copy_(r)
             graphs[kind], pool = g, g.pool()
-        self._graphs, self._out = graphs, out
+        self._graphs, self._out = graphs, (outs[0] if c["head"] is None else outs)
         self.reset()
 
     def _step_captured(self, mlvl_feats, img_metas, can_bus, lidar2img):
@@ -224,5 +252,5 @@ class BEVStream:
         first = token != info["scene_token"] or info["prev_bev"] is None or not self.video_test_mode
         info["scene_token"] = token
         self._graphs["first" if first else "cont"].replay()
-        info["prev_bev"] = self._out
+        info["prev_bev"] = self._out if self._cap["head"] is None else self._out[0]
         return self._out

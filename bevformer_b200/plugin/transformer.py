@@ -1,11 +1,11 @@
-"""PerceptionTransformer.get_bev_features on the CUDA encoder.
+"""PerceptionTransformer on the CUDA encoder and decoder.
 
-Drop-in for the BEV half of the reference class of the same name
-(projects/mmdet3d_plugin/bevformer/modules/transformer.py:26-200): same constructor arguments,
-parameter names (``level_embeds``, ``cams_embeds``, ``reference_points``, ``can_bus_mlp.*``,
-``encoder.*``) and ``get_bev_features`` signature / return value.  The object-query decoder half of the
-reference ``forward`` (transformer.py:203-289) is outside this library's scope (SURVEY.md §8f):
-``forward`` says so instead of silently doing something else.
+Drop-in for the reference class of the same name (projects/mmdet3d_plugin/bevformer/modules/transformer.py:26-289):
+same constructor arguments, parameter names (``level_embeds``, ``cams_embeds``, ``reference_points``,
+``can_bus_mlp.*``, ``encoder.*``, ``decoder.*``), ``get_bev_features`` and ``forward`` signatures and return values.
+``forward`` is ``get_bev_features`` followed by the object-query decoder (plugin/decoder.py), the same tail as
+PerceptionTransformerV2; built without a ``decoder`` dict the module is the BEV encoder alone and ``forward``
+raises ``NotImplementedError``.
 
 What changes underneath: the five tensor passes that build the encoder's key/value tensor become one
 kernel per pyramid level (``bevf_flatten_feats``), and the encoder is ``plugin.encoder.BEVFormerEncoder``.
@@ -21,6 +21,7 @@ import torch
 import torch.nn as nn
 
 from .. import ops, precision
+from .linear import linear
 from .registry import TRANSFORMER, _register, build_transformer_layer_sequence
 
 
@@ -32,8 +33,8 @@ class PerceptionTransformer(nn.Module):
         super().__init__()
         self.init_cfg = init_cfg
         self.encoder = build_transformer_layer_sequence(encoder)
-        self.decoder = None
-        self.decoder_cfg = decoder          # kept for inspection; not built (out of scope)
+        self.decoder = build_transformer_layer_sequence(decoder)
+        self.decoder_cfg = decoder
         self.embed_dims = embed_dims
         self.num_feature_levels = num_feature_levels
         self.num_cams = num_cams
@@ -66,7 +67,8 @@ class PerceptionTransformer(nn.Module):
                 nn.init.xavier_uniform_(p)
         for m in self.modules():
             init = getattr(m, "init_weight", None) or (getattr(m, "init_weights", None) if m is not self else None)
-            if init is not None and type(m).__name__ in ("MSDeformableAttention3D", "TemporalSelfAttention"):
+            if init is not None and type(m).__name__ in ("MSDeformableAttention3D", "TemporalSelfAttention",
+                                                         "CustomMSDeformableAttention"):
                 init()
         nn.init.normal_(self.level_embeds)
         nn.init.normal_(self.cams_embeds)
@@ -208,10 +210,60 @@ class PerceptionTransformer(nn.Module):
                             level_start_index=level_start_index, prev_bev=prev_bev, shift=shift,
                             **kwargs)
 
-    def forward(self, *args, **kwargs):
-        raise NotImplementedError(
-            "bevformer_b200.PerceptionTransformer covers get_bev_features (the BEV encoder half); the "
-            "object-query decoder of the reference forward (transformer.py:203-289) is out of scope")
+    def forward(self, mlvl_feats, bev_queries, object_query_embed=None, bev_h=None, bev_w=None,
+                grid_length=[0.512, 0.512], bev_pos=None, reg_branches=None, cls_branches=None, prev_bev=None,
+                **kwargs):
+        """transformer.py:202-289: ``get_bev_features`` (with every keyword it takes, the device-path ``can_bus=`` /
+        ``lidar2img=`` / ``ego_state=`` / ``ego_mode=`` included), then the decoder over ``object_query_embed``
+        (num_query, 2C) = [query_pos | query].  Returns (bev_embed (Nq, bs, C), inter_states, init_reference_out,
+        inter_references_out) in the compute dtype.  On the device path the call neither synchronises nor copies
+        from host memory, so it can be captured in a CUDA graph (BEVStream)."""
+        if self.decoder is None:
+            raise NotImplementedError(
+                "bevformer_b200.PerceptionTransformer was built without a decoder dict: it is the BEV encoder "
+                "(get_bev_features) alone")
+        dec_kwargs = {k: v for k, v in kwargs.items() if k not in _BEV_ONLY_KWARGS}
+        bev_embed = self.get_bev_features(mlvl_feats, bev_queries, bev_h, bev_w, grid_length=grid_length,
+                                          bev_pos=bev_pos, prev_bev=prev_bev, **kwargs)
+        return _decode(self, bev_embed, object_query_embed, bev_h, bev_w, reg_branches, cls_branches, **dec_kwargs)
+
+
+# get_bev_features' device-path arguments: the decoder layers do not see them
+_BEV_ONLY_KWARGS = ("can_bus", "lidar2img", "ego_state", "ego_mode")
+
+
+def _level_tensors(module, bev_h, bev_w, device):
+    """The decoder's one-level spatial_shapes / level_start_index as device tensors, built once per (shape,
+    device): a fresh ``torch.tensor`` per call is a pageable host copy, which a CUDA graph cannot capture."""
+    cache = module.__dict__.setdefault("_decoder_levels", {})
+    key = (int(bev_h), int(bev_w), str(device))
+    if key not in cache:
+        cache[key] = (torch.tensor([[bev_h, bev_w]], device=device), torch.tensor([0], device=device))
+    return cache[key]
+
+
+@precision.entry("bev_embed", "object_query_embed")
+def _decode(module, bev_embed, object_query_embed, bev_h, bev_w, reg_branches=None, cls_branches=None, **kwargs):
+    """The object-query half of PerceptionTransformer.forward (transformer.py:262-289) and
+    PerceptionTransformerV2.forward (transformerV2.py:329-353): split of ``object_query_embed`` into position and
+    content, initial reference points (Linear + sigmoid), the decoder over ``bev_embed`` (bs, Nq, C).  Returns
+    (bev_embed (Nq, bs, C), inter_states, init_reference_out, inter_references_out)."""
+    bs = bev_embed.shape[0]
+    query_pos, query = torch.split(object_query_embed, module.embed_dims, dim=1)
+    query_pos = query_pos.unsqueeze(0).expand(bs, -1, -1)
+    query = query.unsqueeze(0).expand(bs, -1, -1)
+    rp = module.reference_points
+    reference_points = linear(query_pos, rp.weight, rp.bias).sigmoid()
+    init_reference_out = reference_points
+    query = query.permute(1, 0, 2)
+    query_pos = query_pos.permute(1, 0, 2)
+    bev_embed = bev_embed.permute(1, 0, 2)
+    spatial_shapes, level_start_index = _level_tensors(module, bev_h, bev_w, query.device)
+    inter_states, inter_references = module.decoder(
+        query=query, key=None, value=bev_embed, query_pos=query_pos, reference_points=reference_points,
+        reg_branches=reg_branches, cls_branches=cls_branches, spatial_shapes=spatial_shapes,
+        level_start_index=level_start_index, **kwargs)
+    return bev_embed, inter_states, init_reference_out, inter_references
 
 
 class PerceptionTransformerBEVEncoder(nn.Module):
@@ -401,21 +453,7 @@ class PerceptionTransformerV2(PerceptionTransformerBEVEncoder):
             maps = [x.reshape(x.shape[0], bev_h, bev_w, x.shape[-1]).permute(0, 3, 1, 2).contiguous()
                     for x in prev_bev]
             bev_embed = self.fusion(maps)
-        bs = mlvl_feats[0].size(0)
-        query_pos, query = torch.split(object_query_embed, self.embed_dims, dim=1)
-        query_pos = query_pos.unsqueeze(0).expand(bs, -1, -1)
-        query = query.unsqueeze(0).expand(bs, -1, -1)
-        reference_points = self.reference_points(query_pos).sigmoid()
-        init_reference_out = reference_points
-        query = query.permute(1, 0, 2)
-        query_pos = query_pos.permute(1, 0, 2)
-        bev_embed = bev_embed.permute(1, 0, 2)
-        inter_states, inter_references = self.decoder(
-            query=query, key=None, value=bev_embed, query_pos=query_pos, reference_points=reference_points,
-            reg_branches=reg_branches, cls_branches=cls_branches,
-            spatial_shapes=torch.tensor([[bev_h, bev_w]], device=query.device),
-            level_start_index=torch.tensor([0], device=query.device), **kwargs)
-        return bev_embed, inter_states, init_reference_out, inter_references
+        return _decode(self, bev_embed, object_query_embed, bev_h, bev_w, reg_branches, cls_branches, **kwargs)
 
 
 def patch_reference(cls):

@@ -424,6 +424,32 @@ BEVF_API int bevf_tsa_prep_backward(const float *raw, const float *grad_loc, con
                                     int M, int L, int P, int interleave, void *stream);
 
 /*
+ * The same preparation for F in {1, 2} frames (queue entries); bevf_tsa_prep_* are the F = 2 calls, and the
+ * decoder's CustomMSDeformableAttention (decoder.py:300-330: softmax over L*P, offset / (W, H) + reference point)
+ * is F = 1.
+ *   raw    (B*Nq, M*F*L*P*3) f32: [offsets (M,F,L,P,2) | logits (M,F,L*P)]
+ *   ref2d  (B*F, Nq, L, 2) f32
+ *   loc    (B*F, Nq, M, L, P, 2) f32 out     attn (B*F, Nq, M, L, P) f32 out   (interleave: rows (b, q, frame))
+ *   d_raw  (B*Nq, M*F*L*P*3) as out_dtype (f32, bf16 or f16), fully overwritten.
+ */
+BEVF_API int bevf_query_prep_forward(const float *raw, const float *ref2d, const int64_t *level_hw,
+                                     float *loc, float *attn, int B, int Nq, int M, int L, int P, int F,
+                                     int interleave, void *stream);
+BEVF_API int bevf_query_prep_backward(const float *raw, const float *grad_loc, const float *grad_attn,
+                                      const int64_t *level_hw, void *d_raw, int out_dtype, int B, int Nq, int M,
+                                      int L, int P, int F, int interleave, void *stream);
+
+/*
+ * Reference-point refinement of DetectionTransformerDecoder (decoder.py:106-118), forward only (the result is
+ * detached):  out[r, c] = sigmoid(tmp[r, col_c] + inverse_sigmoid(ref[r, c])), col = (0, 1, 4), eps = 1e-5.
+ *   tmp    (rows, >= 5) rows tmp_row_stride elements apart (the regression branch output, read in place)
+ *   ref    (rows, 3) contiguous     out (rows, 3) contiguous; tmp, ref, out all in `dtype` (f32 | bf16 | f16)
+ *   ref2d  optional (rows, 2) f32 out: the x, y of `out`, the next layer's sampling-point prep input
+ */
+BEVF_API int bevf_refine_points(const void *tmp, int64_t tmp_row_stride, const void *ref, void *out, float *ref2d,
+                                int dtype, int64_t rows, void *stream);
+
+/*
  * y = LayerNorm(dropout(x) + residual) * gamma + beta, optionally also y_plus_pos = y + pos.
  * replaces the `norm` steps of BEVFormerLayer.forward (encoder.py:377-379) together with the
  * preceding "self.dropout(output) + identity" of the attention / FFN
