@@ -61,8 +61,6 @@ SIGNATURES = {
     "bevf_msda_dense_plan": (c_int, [c_void_p, c_int, c_int, c_int, c_void_p, c_int, c_void_p]),
     "bevf_sca_plan_workspace_ints": (c_int64, [c_int, c_int]),
     "bevf_sca_plan_build": (c_int, [c_void_p] * 10 + [c_int] * 5 + [c_void_p]),
-    "bevf_msda_rows_forward_staged": (c_int, [c_void_p, c_int, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p,
-                                              c_void_p, c_int, c_void_p] + [c_int] * 7 + [c_void_p]),
     "bevf_sca_prep_forward": (c_int, [c_void_p] * 7 + [c_int] * 8 + [c_void_p]),
     "bevf_sca_prep_backward": (c_int, [c_void_p] * 6 + [c_int] * 8 + [c_void_p]),
     "bevf_sca_rows_forward_fused": (c_int, [c_void_p, c_int] + [c_void_p] * 9 + [c_int, c_void_p, c_int, c_void_p]
@@ -165,7 +163,7 @@ def load(build_if_missing: bool = True):
     return _lib
 
 
-ABI_VERSION = 1
+ABI_VERSION = 2
 
 
 def check(status: int, lib=None) -> None:

@@ -618,15 +618,10 @@ msda_bwd_generic(const T *__restrict__ value, const int64_t *__restrict__ level_
 // ------------------------------------------------------------------------------------------------
 // host launchers
 // ------------------------------------------------------------------------------------------------
-// row groups handled per warp: 1; BEVF_MSDA_ITERS overrides (experiments).
-static int pick_iters(long long rows, int G) {
-    static int forced = -1;
-    if (forced < 0) {
-        const char *e = getenv("BEVF_MSDA_ITERS");
-        forced = e ? atoi(e) : 0;
-    }
-    (void)rows; (void)G;
-    return forced > 0 ? forced : 1;   // >1 loses parallelism for no L1 gain
+// The head_dim 32 kernels take one group of G rows per warp (iters = 1): more loses parallelism for no L1 gain.
+static unsigned grid_d32(long long rows, int G) {
+    const long long per_block = (long long)(kThreads / 32) * G;
+    return (unsigned)((rows + per_block - 1) / per_block);
 }
 
 static int check_dims(const char *who, int B, int S, int M, int D, int Q, int L, int P) {
@@ -645,20 +640,17 @@ static int launch_fwd(const char *who, const void *value, const int64_t *hw, con
                       int M, int D, int Q, int L, int P, long long rows, cudaStream_t st,
                       const ScaFuse *fz = nullptr) {
     if (D == 32) {
-        constexpr int G = Vec<T>::N;      // rows per warp == channels per lane (4 or 8)
-        const int iters = pick_iters(rows, G);
-        const long long per_block = (long long)(kThreads / 32) * G * iters;
-        const unsigned grid = (unsigned)((rows + per_block - 1) / per_block);
+        const unsigned grid = grid_d32(rows, Vec<T>::N);
         if (fz) {
             if constexpr (std::is_same<T, bf16>::value && std::is_same<TO, bf16>::value)
                 msda_fwd_d32<T, TO, true><<<grid, kThreads, 0, st>>>((const T *)value, hw, ls, nullptr, nullptr, (TO *)out,
-                                                                     row_map, S, M, Q, L, P, (65536 + P - 1) / P, iters,
+                                                                     row_map, S, M, Q, L, P, (65536 + P - 1) / P, 1,
                                                                      rows, *fz);
             else
                 return fail("%s: the fused prep needs bf16 value and output", who);
         } else {
             msda_fwd_d32<T, TO><<<grid, kThreads, 0, st>>>((const T *)value, hw, ls, loc, attn, (TO *)out,
-                                                           row_map, S, M, Q, L, P, (65536 + P - 1) / P, iters,
+                                                           row_map, S, M, Q, L, P, (65536 + P - 1) / P, 1,
                                                            rows);
         }
     } else if (fz) {
@@ -773,13 +765,10 @@ static int launch_bwd(const char *who, const void *value, const int64_t *hw, con
         // fixed-point grad_value: always the one-kernel backward (the split / hybrid / dense modes sum in fp32)
         long long *gfx = reinterpret_cast<long long *>(gv);
         if (D == 32) {
-            constexpr int G = Vec<T>::N;
-            const int iters = pick_iters(rows, G);
-            const long long per_block = (long long)(kThreads / 32) * G * iters;
-            const unsigned grid = (unsigned)((rows + per_block - 1) / per_block);
+            const unsigned grid = grid_d32(rows, Vec<T>::N);
             msda_bwd_d32<T, TG, true, long long><<<grid, kThreads, 0, st>>>(
                 (const T *)value, hw, ls, loc, attn, (const TG *)go, gfx, gl, ga, row_map, S, M, Q, L, P,
-                (65536 + P - 1) / P, iters, rows, 0u, hl, nullptr, nullptr, 0u, 0, 0, fx->bounds, fx->frac_bits);
+                (65536 + P - 1) / P, 1, rows, 0u, hl, nullptr, nullptr, 0u, 0, 0, fx->bounds, fx->frac_bits);
         } else {
             const unsigned grid = (unsigned)((rows + kThreads / 32 - 1) / (kThreads / 32));
             msda_bwd_generic<T, TG, long long><<<grid, kThreads, 0, st>>>(
@@ -792,13 +781,10 @@ static int launch_bwd(const char *who, const void *value, const int64_t *hw, con
         // grad_value stored and accumulated in scaled fp16: bf16 value rows, head_dim 32, the one-kernel backward only
         if constexpr (std::is_same<T, bf16>::value) {
             if (D != 32) return fail("%s: fp16 grad_value needs head_dim 32", who);
-            constexpr int G = Vec<T>::N;
-            const int iters = pick_iters(rows, G);
-            const long long per_block = (long long)(kThreads / 32) * G * iters;
-            const unsigned grid = (unsigned)((rows + per_block - 1) / per_block);
+            const unsigned grid = grid_d32(rows, Vec<T>::N);
             msda_bwd_d32<T, TG, true, __half><<<grid, kThreads, 0, st>>>((const T *)value, hw, ls, loc, attn, (const TG *)go,
                                                                        reinterpret_cast<__half *>(gv), gl, ga, row_map, S, M,
-                                                                       Q, L, P, (65536 + P - 1) / P, iters, rows, 0u, hl,
+                                                                       Q, L, P, (65536 + P - 1) / P, 1, rows, 0u, hl,
                                                                        mixed ? mixed->amax : nullptr);
             return check_launch(who);
         } else {
@@ -808,22 +794,19 @@ static int launch_bwd(const char *who, const void *value, const int64_t *hw, con
     if (mixed && mixed->gv16) {
         if constexpr (std::is_same<T, bf16>::value) {
             if (D != 32) return fail("%s: mixed accumulation needs head_dim 32", who);
-            constexpr int G = Vec<T>::N;
-            const int iters = pick_iters(rows, G);
-            const long long per_block = (long long)(kThreads / 32) * G * iters;
-            const unsigned grid = (unsigned)((rows + per_block - 1) / per_block);
+            const unsigned grid = grid_d32(rows, Vec<T>::N);
             if (fz) {
                 if constexpr (std::is_same<TG, bf16>::value)
                     msda_bwd_d32<T, TG, true, float, true><<<grid, kThreads, 0, st>>>(
                         (const T *)value, hw, ls, nullptr, nullptr, (const TG *)go, gv, gl, ga, row_map, S, M, Q, L, P,
-                        (65536 + P - 1) / P, iters, rows, done_levels, hl, mixed->amax, mixed->gv16, mixed->mask,
+                        (65536 + P - 1) / P, 1, rows, done_levels, hl, mixed->amax, mixed->gv16, mixed->mask,
                         mixed->side_start, mixed->S_side, nullptr, 0, *fz);
                 else
                     return fail("%s: the fused prep needs a bf16 grad_out", who);
                 return check_launch(who);
             }
             msda_bwd_d32<T, TG, true><<<grid, kThreads, 0, st>>>((const T *)value, hw, ls, loc, attn, (const TG *)go, gv, gl, ga,
-                                                               row_map, S, M, Q, L, P, (65536 + P - 1) / P, iters, rows,
+                                                               row_map, S, M, Q, L, P, (65536 + P - 1) / P, 1, rows,
                                                                done_levels, hl, mixed->amax, mixed->gv16, mixed->mask, mixed->side_start,
                                                                mixed->S_side);
             return check_launch(who);
@@ -832,10 +815,7 @@ static int launch_bwd(const char *who, const void *value, const int64_t *hw, con
         }
     }
     if (D == 32) {
-        constexpr int G = Vec<T>::N;
-        const int iters = pick_iters(rows, G);
-        const long long per_block = (long long)(kThreads / 32) * G * iters;
-        const unsigned grid = (unsigned)((rows + per_block - 1) / per_block);
+        const unsigned grid = grid_d32(rows, Vec<T>::N);
         const int mode = done_levels ? 0 : bwd_split_enabled();
         if (mode != 0 && std::is_same<T, __half>::value)
             return fail("%s: the split / hybrid backward modes take fp32 or bf16 only (fp16 needs mode 0)", who);
@@ -846,7 +826,7 @@ static int launch_bwd(const char *who, const void *value, const int64_t *hw, con
                 return e;
             msda_bwd_d32<T, TG, false><<<grid, kThreads, 0, st>>>((const T *)value, hw, ls, loc, attn,
                                                                   (const TG *)go, gv, gl, ga, row_map, S, M,
-                                                                  Q, L, P, (65536 + P - 1) / P, iters, rows, 0u, hl);
+                                                                  Q, L, P, (65536 + P - 1) / P, 1, rows, 0u, hl);
         } else if (mode == 2 && can_split && L >= 2 && g_side_stream) {
             // hybrid: the coarse half of the pyramid (most collisions, 47 % of the reduction bytes at base)
             // through the register-merging splat on the second stream, everything else in the one-kernel
@@ -863,12 +843,12 @@ static int launch_bwd(const char *who, const void *value, const int64_t *hw, con
             cudaEventRecord(join, g_side_stream);
             msda_bwd_d32<T, TG, true><<<grid, kThreads, 0, st>>>((const T *)value, hw, ls, loc, attn,
                                                                  (const TG *)go, gv, gl, ga, row_map, S, M,
-                                                                 Q, L, P, (65536 + P - 1) / P, iters, rows, coarse, hl);
+                                                                 Q, L, P, (65536 + P - 1) / P, 1, rows, coarse, hl);
             cudaStreamWaitEvent(st, join, 0);
         } else {
             msda_bwd_d32<T, TG, true><<<grid, kThreads, 0, st>>>((const T *)value, hw, ls, loc, attn,
                                                                  (const TG *)go, gv, gl, ga, row_map, S, M,
-                                                                 Q, L, P, (65536 + P - 1) / P, iters, rows, done_levels, hl);
+                                                                 Q, L, P, (65536 + P - 1) / P, 1, rows, done_levels, hl);
         }
     } else {
         const unsigned grid = (unsigned)((rows + kThreads / 32 - 1) / (kThreads / 32));

@@ -1,4 +1,4 @@
-// Device helpers shared by the sampler kernels (msda.cu, msda_splat.cuh, msda_staged.cu): the bilinear
+// Device helpers shared by the sampler kernels (msda.cu, msda_splat.cuh, msda_dense.cu): the bilinear
 // corner arithmetic of SURVEY.md Appendix A, the 16-byte row slices and their fp32 / bf16 math.
 #pragma once
 
@@ -268,12 +268,6 @@ __device__ __forceinline__ float2 sca_row_stats(const ScaRow &sr, bool live, int
 #pragma unroll
     for (int i = 0; i < 8; ++i) a[i] *= inv;
     return make_float2(mx, inv);
-}
-
-template <typename T> __device__ __forceinline__ decltype(Vec<T>::v) vec_bits(const uint4 &u);
-template <> __device__ __forceinline__ uint4 vec_bits<bf16>(const uint4 &u) { return u; }
-template <> __device__ __forceinline__ float4 vec_bits<float>(const uint4 &u) {
-    return make_float4(__uint_as_float(u.x), __uint_as_float(u.y), __uint_as_float(u.z), __uint_as_float(u.w));
 }
 
 }  // namespace bevf

@@ -250,33 +250,6 @@ def msda_rows_forward(value, spatial_shapes, level_start_index, loc, attn, row_m
     return out
 
 
-def msda_rows_forward_staged(value, spatial_shapes, level_start_index, level_hw_host, loc, attn, map_range,
-                             out_dtype=None):
-    """msda_rows_forward for row lists grouped by value map, coarse levels TMA-staged in shared memory
-    (bevf_msda_rows_forward_staged).  level_hw_host: [(h, w), ...] python ints; map_range (NB, 2) int32."""
-    import ctypes
-    for t, n in ((value, "value"), (loc, "sampling_loc"), (attn, "attn_weight"), (map_range, "map_range")):
-        _need_cuda(t, n)
-    if value.dtype not in _DT or loc.dtype != torch.float32 or attn.dtype != torch.float32:
-        raise RuntimeError("value must be float32/bfloat16/float16, sampling_loc and attn_weight float32")
-    NB, S, M, D = value.shape
-    R, M2, L, P, _ = loc.shape
-    if M2 != M or tuple(attn.shape) != (R, M, L, P) or map_range.numel() != 2 * NB or len(level_hw_host) != L:
-        raise RuntimeError("value / sampling_loc / attn_weight / map_range / level shapes disagree")
-    ss, ls = _level_tensors(value, spatial_shapes, level_start_index)
-    hw = (ctypes.c_int32 * (2 * L))(*[int(v) for hw_ in level_hw_host for v in hw_])
-    out_dtype = out_dtype or value.dtype
-    out = torch.empty((R, M * D), device=value.device, dtype=out_dtype)
-    lib = _lib.load()
-    with torch.cuda.device(value.device), _timed("msda_rows_forward", value.device, (R, L)):
-        st = lib.bevf_msda_rows_forward_staged(value.data_ptr(), _DT[value.dtype], ss.data_ptr(), ls.data_ptr(),
-                                               ctypes.addressof(hw), loc.data_ptr(), attn.data_ptr(),
-                                               out.data_ptr(), _DT[out_dtype], map_range.data_ptr(),
-                                               NB, S, M, D, R, L, P, _stream_ptr(value))
-    _lib.check(st, lib)
-    return out
-
-
 _DENSE_INIT = [False]
 
 
@@ -586,42 +559,19 @@ class SamplerRows(Function):
 
     @staticmethod
     def forward(ctx, value, loc, attn, row_map, spatial_shapes, level_start_index, group_order=None,
-                staged=None, gv_mode=None):
-        """``staged`` = (level_hw_host, map_range): use the TMA-staged forward (rows grouped by value map).
-        An fp16 ``value`` is read natively (no widened copy); the staged, dense and fp16-accumulating variants take
-        bf16 / fp32 only and are skipped for it."""
+                dense=None, gv_mode=None):
+        """``dense`` = (level_hw_host, map_range) for rows grouped by value map: the backward may hand the coarse
+        levels' grad_value to the dense tensor-core kernel.  An fp16 ``value`` is read natively (no widened copy);
+        the dense and fp16-accumulating variants take bf16 / fp32 only and are skipped for it."""
         half = value.dtype == torch.float16
-        # an alternative to the plain kernel, opt-in for A/B runs
-        if (staged is not None and not half and value.shape[-1] == 32
-                and os.environ.get("BEVF_MSDA_FWD", "plain") == "staged"):
-            out = msda_rows_forward_staged(value, spatial_shapes, level_start_index, staged[0], loc, attn,
-                                           staged[1])
-        else:
-            out = msda_rows_forward(value, spatial_shapes, level_start_index, loc, attn, row_map)
+        out = msda_rows_forward(value, spatial_shapes, level_start_index, loc, attn, row_map)
         ctx.save_for_backward(value, loc, attn, row_map, spatial_shapes, level_start_index)
         ctx.group_order = group_order
         # grad_value accumulated in scaled fp16 -- "f16": every level, ("mixed", level_hw_host, n): the first n levels
         # -- (half the L2 reduction sectors of those levels): only where the caller asks for it
         ctx.gv_mode = gv_mode if (gv_mode is not None and value.dtype == torch.bfloat16 and value.shape[-1] == 32) else None
-        ctx.dense = staged if (staged is not None and not half and value.shape[-1] == 32) else None
+        ctx.dense = dense if (dense is not None and not half and value.shape[-1] == 32) else None
         ctx.value_early = getattr(value, "_bevf_early", None)     # see plugin/linear.py::shared_input_projections
-        ctx.gv_zero = None
-        aux = aux_stream(value.device)
-        if (aux is not None and value.requires_grad and torch.is_grad_enabled()
-                and os.environ.get("BEVF_AUX_FILL", "0") == "1"):
-            # the backward accumulates grad_value into a zero-filled fp32 buffer: fill it NOW on the second
-            # stream (it overlaps the forward) instead of on the backward's critical path.  It holds 1.6 GB from
-            # forward to backward: opt-in (BEVF_AUX_FILL=1)
-            main = torch.cuda.current_stream(value.device)
-            ev = torch.cuda.Event()
-            ev.record(main)
-            aux.wait_event(ev)
-            with torch.cuda.stream(aux):
-                gv0 = torch.zeros(value.shape, device=value.device, dtype=torch.float32)
-                done = torch.cuda.Event()
-                done.record(aux)
-            gv0.record_stream(main)
-            ctx.gv_zero = (gv0, done)
         return out
 
     @staticmethod
@@ -629,17 +579,12 @@ class SamplerRows(Function):
     def backward(ctx, grad_out):
         value, loc, attn, row_map, ss, ls = ctx.saved_tensors
         if deterministic():
-            # fixed-point grad_value; gv_mode, the dense / split kernels and the pre-filled fp32 buffer all sum in
-            # floating point and are bypassed
+            # fixed-point grad_value; gv_mode and the dense / split kernels sum in floating point and are bypassed
             gv, gl, ga = msda_backward_fx(value, ss, ls, loc, attn, grad_out.contiguous(), row_map)
             if ctx.value_early is not None and ctx.value_early(gv):
                 return None, gl, ga, None, None, None, None, None, None      # converted off the critical path
             return gv.materialize(), gl, ga, None, None, None, None, None, None
-        gv0 = None
-        if ctx.gv_zero is not None:
-            gv0, done = ctx.gv_zero
-            torch.cuda.current_stream(value.device).wait_event(done)
-        if ctx.gv_mode is not None and gv0 is None and grad_out.dtype == torch.bfloat16:
+        if ctx.gv_mode is not None and grad_out.dtype == torch.bfloat16:
             if ctx.gv_mode == "f16":
                 gv, gl, ga = msda_rows_backward_f16acc(value, ss, ls, loc, attn, row_map, grad_out, ctx.group_order,
                                                        lazy=True)
@@ -668,7 +613,7 @@ class SamplerRows(Function):
             return gv.materialize(), gl, ga, None, None, None, None, None, None
         # (the coarse levels of an fp32-accumulated pyramid go to the dense kernel only where the caller opted in:
         # bevf_msda_rows_backward_dense is off under the library default)
-        gv, gl, ga = msda_rows_backward(value, ss, ls, loc, attn, row_map, grad_out.contiguous(), gv0,
+        gv, gl, ga = msda_rows_backward(value, ss, ls, loc, attn, row_map, grad_out.contiguous(),
                                         group_order=ctx.group_order, dense=ctx.dense)
         if ctx.value_early is not None and ctx.value_early(gv):
             # the producer of `value` took the gradient (conversion + its GEMMs run off the critical path)

@@ -528,10 +528,10 @@ class BEVFormerEncoder(nn.Module):
         return self._grad_arena
 
     def _level_shapes_host(self, spatial_shapes):
-        """[(h, w), ...] as python ints, for the TMA tensor maps of the staged sampler.  Lists / CPU tensors
+        """[(h, w), ...] as python ints, for ops.gv_mode_for and the dense sampler backward.  Lists / CPU tensors
         are read directly; a device tensor is read ONCE (one sync, never during a graph capture) and
-        remembered by its storage address -- safe to go stale, because the kernel re-checks the shapes
-        against the device tensor and falls back to the unstaged path on a mismatch."""
+        remembered by its storage address -- safe to go stale, because the sampler backward re-checks the
+        shapes against the device tensor and leaves the levels to the reduction path on a mismatch."""
         if not torch.is_tensor(spatial_shapes):
             return [(int(h), int(w)) for h, w in spatial_shapes]
         if not spatial_shapes.is_cuda:

@@ -204,25 +204,22 @@ class SpatialCrossAttention(nn.Module):
         nn.init.xavier_uniform_(self.output_proj.weight)
         nn.init.zeros_(self.output_proj.bias)
 
-    def _fused_prep(self, query, w, v, gv_mode, staged) -> bool:
+    def _fused_prep(self, query, w, v, gv_mode, dense) -> bool:
         """Whether the sampler computes the sampling points itself (plugin/linear.py::sca_head_sampler): the 16-bit
         tensor-core head, 8 heads of 32 channels and 32 samples per head, the mixed grad_value accumulation with a
-        host pyramid that matches the value maps, outside deterministic mode (its fixed-point backward reads loc /
-        attn) and unless the staged forward or the pre-filled fp32 grad_value buffer (opt-in A/B paths of
-        ops.SamplerRows) was asked for."""
+        host pyramid that matches the value maps, and outside deterministic mode (its fixed-point backward reads loc /
+        attn)."""
         da = self.deformable_attention
-        return (isinstance(gv_mode, tuple) and staged is not None and not ops.deterministic()
+        return (isinstance(gv_mode, tuple) and dense is not None and not ops.deterministic()
                 and da.num_heads == 8 and v.shape[-1] == 32 and da.num_levels * da.num_points == 32
-                and use_tc(query, w) and sum(h * w_ for h, w_ in gv_mode[1]) == v.shape[1]
-                and os.environ.get("BEVF_MSDA_FWD", "plain") != "staged"
-                and os.environ.get("BEVF_AUX_FILL", "0") != "1")
+                and use_tc(query, w) and sum(h * w_ for h, w_ in gv_mode[1]) == v.shape[1])
 
     def attend(self, query, value, reference_points_cam, bev_mask, spatial_shapes,
                level_start_index, plan: Optional[ScaPlan] = None, level_hw_host=None, value_pre=None):
         """Everything up to and including output_proj, WITHOUT dropout / residual.
         query (bs, Nq, C); value (num_cams, S, bs, C).  ``level_hw_host``: [(h, w), ...] python ints of
-        the pyramid, when the caller knows them without a device read: the sampler forward then stages
-        the coarse levels in shared memory through TMA.  ``value_pre``: value_proj(value) already computed
+        the pyramid, when the caller knows them without a device read: the sampler backward then picks
+        its grad_value accumulation per level (ops.gv_mode_for) and hands the coarse levels to the dense kernel.  ``value_pre``: value_proj(value) already computed
         by the encoder for all layers at once (plugin/linear.py::shared_input_projections)."""
         da = self.deformable_attention
         bs, nq, c = query.shape
@@ -246,14 +243,14 @@ class SpatialCrossAttention(nn.Module):
         v = value_pre.view(bs * ncam, s, m, -1)
         if hasattr(value_pre, "_bevf_early"):
             v._bevf_early = value_pre._bevf_early
-        staged = None
+        dense = None
         if level_hw_host is not None and plan.map_range is not None and len(level_hw_host) == l:
-            staged = (level_hw_host, plan.map_range)
+            dense = (level_hw_host, plan.map_range)
         # grad_value of the fine pyramid levels accumulated in scaled fp16, the coarse ones in fp32 (ops.gv_mode_for)
         gv_mode = None
         if level_hw_host is not None and len(level_hw_host) == l and v.dtype == torch.bfloat16:
             gv_mode = ops.gv_mode_for(plan.row_map.numel() / max(1, bs * ncam), p, level_hw_host)
-        if self._fused_prep(query, w, v, gv_mode, staged):
+        if self._fused_prep(query, w, v, gv_mode, dense):
             # the sampling-point prep inside the sampler kernels: loc / attn never go through memory
             fuse = (plan.ref_cam, plan.pair_q, plan.pair_cam, plan.pair_of, plan.row_map, ss, lsi, bs, nq,
                     gv_mode[1], gv_mode[2], plan.map_range)
@@ -261,7 +258,7 @@ class SpatialCrossAttention(nn.Module):
         else:
             loc, attn = sca_sampling_head(query, w, b, plan.ref_cam, plan.pair_q, plan.pair_cam,
                                           plan.pair_of, ss, bs, nq, m, l, p)
-            out = ops.SamplerRows.apply(v, loc, attn, plan.row_map, ss, lsi, None, staged, gv_mode)   # (bs*R, C)
+            out = ops.SamplerRows.apply(v, loc, attn, plan.row_map, ss, lsi, None, dense, gv_mode)   # (bs*R, C)
         slots = ops.ScaCombine.apply(out, plan.pair_of, plan.pair_q, plan.inv_count, bs, nq)
         return linear(slots, self.output_proj.weight, self.output_proj.bias)
 

@@ -40,7 +40,7 @@
 extern "C" {
 #endif
 
-#define BEVF_ABI_VERSION 1
+#define BEVF_ABI_VERSION 2
 
 #if defined(__GNUC__)
 #define BEVF_API __attribute__((visibility("default")))
@@ -245,24 +245,6 @@ BEVF_API int bevf_msda_fx_convert(const int64_t *grad_value_fx, const uint32_t *
                                   int out_dtype, int accumulate, int64_t n, void *stream);
 
 /*
- * bevf_msda_rows_forward with the coarse pyramid levels staged in shared memory by TMA.
- * For row lists whose rows are grouped by value map (the SCA pair list: camera-major): a CTA takes one
- * (value map, head) and a share of that map's rows, loads every level that fits -- coarsest first, whole
- * level of that head, one cp.async.bulk.tensor per level -- and gathers those levels from shared memory;
- * finer levels keep the global path.  Same results as bevf_msda_rows_forward.
- *   level_hw_host  (L, 2) int32 HOST copy of level_hw (the tensor maps are built on the host); a level
- *                  whose host shape disagrees with the device-side level_hw / level_start is not staged
- *   map_range      (B, 2) int32 DEVICE: [first, end) rows of every value map (bevf_sca_plan_build)
- *   B = number of value maps; levels must be stored back to back (level_start[l] = sum of H*W before l,
- *   the reference's own definition, transformer.py:178-180); head_dim 32; fp32 or bf16 only (fp16 is an error).
- */
-BEVF_API int bevf_msda_rows_forward_staged(const void *value, int value_dtype, const int64_t *level_hw,
-                                           const int64_t *level_start, const int32_t *level_hw_host,
-                                           const float *loc, const float *attn, void *out, int out_dtype,
-                                           const int32_t *map_range, int B, int S, int M, int D, int R,
-                                           int L, int P, void *stream);
-
-/*
  * bevf_msda_rows_backward for row lists grouped by value map (the SCA pair list), with grad_value of the
  * COARSE pyramid levels computed as a dense product on the tensor cores (csrc/msda_dense.cu) instead of one
  * L2 reduction per (sample, corner): for a (value map, head) the col2im scatter of
@@ -329,7 +311,7 @@ BEVF_API int bevf_msda_set_backward_mode(int mode);
  *   row_map    (B*capacity,) int32       out; value map b*ncam+cam of sampler row b*capacity+r, -1 = unused
  *   inv_count  (B, Nq) f32               out; 1 / max(1, #cameras seeing q in batch item b)  (:169-171)
  *   map_range  (B*ncam, 2) int32         out; [first, end) sampler rows of value map b*ncam+cam (its rows are
- *                                        contiguous) -- what bevf_msda_rows_forward_staged partitions by
+ *                                        contiguous) -- what bevf_msda_rows_backward_dense partitions by
  *   counters   (2,) int32                out; [0] = number of pairs found, [1] = 1 if it exceeded capacity
  *                                        (the pairs beyond capacity are dropped: the caller must check)
  *   workspace  bevf_sca_plan_workspace_ints(ncam, Nq) int32
