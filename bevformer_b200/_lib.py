@@ -126,6 +126,12 @@ SIGNATURES = {
     "bevf_ego_motion": (c_int, [c_void_p, c_void_p, c_int, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int]
                         + [ctypes.c_double] * 4 + [c_int, c_void_p]),
     "bevf_rotate_bev": (c_int, [c_void_p, c_int, c_int64, c_int64, c_void_p, c_void_p] + [c_int] * 5 + [c_void_p]),
+    "bevf_det_branches_forward": (c_int, [c_void_p, c_int64, c_int64, c_int64, c_int, c_void_p, c_void_p, c_int,
+                                          c_void_p, c_int, c_void_p, c_void_p] + [c_int] * 6
+                                  + [ctypes.c_float, c_void_p, c_void_p]),
+    "bevf_nms_free_decode": (c_int, [c_void_p, c_int, c_void_p, c_int] + [c_int] * 5
+                             + [c_void_p, c_int, ctypes.c_double, c_int] + [c_void_p] * 5),
+    "bevf_nms_free_decode_smem_bytes": (c_int64, [c_int, c_int, c_int]),
 }
 
 
@@ -163,7 +169,7 @@ def load(build_if_missing: bool = True):
     return _lib
 
 
-ABI_VERSION = 2
+ABI_VERSION = 3
 
 
 def check(status: int, lib=None) -> None:

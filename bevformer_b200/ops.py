@@ -1538,3 +1538,142 @@ class GroupAttention(Function):
         if stacked:
             return dqk, None, dv, None, None, None, None
         return dq, dk, dv, None, None, None, None
+
+
+# ---------------------------------------------------------------------------------------------------
+# Detection head (csrc/det_head.cu): BEVFormerHead's branch MLPs for every decoder level in one launch, and
+# NMSFreeCoder's decode without host synchronisation.
+# ---------------------------------------------------------------------------------------------------
+def det_branch_params(cls_branch, reg_branch):
+    """The 16 parameter tensors of one level's (cls, reg) branch pair, in the order bevf_det_branches_forward reads
+    them.  The branches must have BEVFormerHead's layout with num_reg_fcs = 2: cls = Linear-LayerNorm-ReLU x 2 +
+    Linear, reg = Linear-ReLU x 2 + Linear."""
+    import torch.nn as nn
+    c, r = list(cls_branch), list(reg_branch)
+    kinds_c = [nn.Linear, nn.LayerNorm, nn.ReLU] * 2 + [nn.Linear]
+    kinds_r = [nn.Linear, nn.ReLU] * 2 + [nn.Linear]
+    if len(c) != 7 or len(r) != 5 or not all(isinstance(m, k) for m, k in zip(c + r, kinds_c + kinds_r)):
+        raise NotImplementedError("det_branches_forward: the fused branches need BEVFormerHead's layout with "
+                                  "num_reg_fcs=2 (Linear-LayerNorm-ReLU x 2 + Linear / Linear-ReLU x 2 + Linear)")
+    if any(m.bias is None for m in (c[0], c[3], c[6], r[0], r[2], r[4])) or not (c[1].elementwise_affine
+                                                                               and c[4].elementwise_affine):
+        raise NotImplementedError("det_branches_forward: Linear layers need a bias and LayerNorms an affine transform")
+    return [c[0].weight, c[0].bias, c[1].weight, c[1].bias, c[3].weight, c[3].bias, c[4].weight, c[4].bias,
+            c[6].weight, c[6].bias, r[0].weight, r[0].bias, r[2].weight, r[2].bias, r[4].weight, r[4].bias]
+
+
+def det_branches_forward(states, init_reference, inter_references, level_params, pc_range, ln_eps=1e-5):
+    """BEVFormerHead.forward after the transformer (bevformer_head.py:171-203) for every level in one launch.
+
+    states            (L, nq, bs, 256) bf16 / fp16 decoder states, read through their strides (channels contiguous)
+    init_reference    (bs, nq, 3), inter_references (L, bs, nq, 3): fp32 or the states' dtype
+    level_params      L lists of ``det_branch_params``; all in the states' dtype or all fp32 (autocast: fp32 weights
+                      and Linear biases are rounded to the states' dtype inside the kernel, as autocast's Linear
+                      rounds them; LayerNorm parameters are read in fp32)
+    pc_range          6 numbers
+    Returns (all_cls_scores (L, bs, nq, ncls), all_bbox_preds (L, bs, nq, 10)) in the states' dtype.  No autograd."""
+    if not states.is_cuda:
+        raise RuntimeError("states must be a CUDA tensor (bevformer_b200 has no CPU path)")
+    if states.dtype not in TC_DTYPES:
+        raise RuntimeError(f"det_branches_forward: bf16 or fp16 states only (got {states.dtype})")
+    if states.dim() != 4 or states.shape[3] != 256 or states.stride(3) != 1:
+        raise RuntimeError(f"det_branches_forward: states must be (L, nq, bs, 256) with contiguous channels, got "
+                           f"{tuple(states.shape)}")
+    L, nq, bs, C = states.shape
+    if any(s % 8 for s in states.stride()[:3]) or states.data_ptr() % 16:
+        states = states.contiguous()
+    if len(level_params) != L or not 1 <= L <= 8:
+        raise RuntimeError(f"det_branches_forward: {len(level_params)} parameter sets for {L} levels (1 to 8)")
+    pdt = level_params[0][0].dtype
+    if pdt not in (states.dtype, torch.float32):
+        raise RuntimeError(f"det_branches_forward: parameters in {pdt}; need {states.dtype} or float32")
+    ncls = level_params[0][8].shape[0]
+    shapes = [(C, C), (C,), (C,), (C,), (C, C), (C,), (C,), (C,), (ncls, C), (ncls,),
+              (C, C), (C,), (C, C), (C,), (10, C), (10,)]
+    if not 1 <= ncls <= 16:
+        raise RuntimeError(f"det_branches_forward: {ncls} classes; the kernel takes 1 to 16")
+    ptrs = []
+    for ps in level_params:
+        if len(ps) != 16:
+            raise RuntimeError("det_branches_forward: 16 parameter tensors per level (ops.det_branch_params)")
+        for t, shp in zip(ps, shapes):
+            if tuple(t.shape) != shp:
+                raise RuntimeError(f"det_branches_forward: parameter of shape {tuple(t.shape)}, expected {shp} "
+                                   "(embed_dims 256, code_size 10)")
+            if t.dtype != pdt or t.device != states.device or not t.is_contiguous():
+                raise RuntimeError("det_branches_forward: parameters must be contiguous, on the states' device and "
+                                   "all of one dtype")
+            ptrs.append(t.data_ptr())
+    refs = []
+    for name, r, shp in (("init_reference", init_reference, (bs, nq, 3)),
+                         ("inter_references", inter_references, (L, bs, nq, 3))):
+        if tuple(r.shape) != shp:
+            raise RuntimeError(f"det_branches_forward: {name} of shape {tuple(r.shape)}, expected {shp}")
+        if r.dtype not in _DT:
+            raise RuntimeError(f"det_branches_forward: {name} must be float32, bfloat16 or float16")
+        if r.device != states.device:
+            raise RuntimeError(f"det_branches_forward: {name} must be on the states' device ({states.device})")
+        refs.append(r.to(init_reference.dtype).contiguous())
+    if len(pc_range) != 6:
+        raise RuntimeError("det_branches_forward: pc_range needs 6 numbers")
+    cls = torch.empty((L, bs, nq, ncls), device=states.device, dtype=states.dtype)
+    box = torch.empty((L, bs, nq, 10), device=states.device, dtype=states.dtype)
+    import ctypes
+    table = (ctypes.c_void_p * len(ptrs))(*ptrs)
+    pc = (ctypes.c_double * 6)(*[float(v) for v in pc_range])
+    lib = _lib.load()
+    with torch.cuda.device(states.device):
+        st = lib.bevf_det_branches_forward(states.data_ptr(), states.stride(0), states.stride(1), states.stride(2),
+                                           _DT[states.dtype], refs[0].data_ptr(), refs[1].data_ptr(),
+                                           _DT[refs[0].dtype], ctypes.cast(table, ctypes.c_void_p), _DT[pdt],
+                                           cls.data_ptr(), box.data_ptr(), L, bs, nq, C, ncls, 10, float(ln_eps),
+                                           ctypes.cast(pc, ctypes.c_void_p), _stream_ptr(states))
+    _lib.check(st, lib)
+    return cls, box
+
+
+def nms_free_decode(cls_scores, bbox_preds, max_num, post_center_range, score_threshold=None, z_shift=False):
+    """NMSFreeCoder.decode (nms_free_coder.py:40-121) for a batch in one launch, no host synchronisation.
+
+    cls_scores (bs, nq, ncls) logits, bbox_preds (bs, nq, 10) normalised boxes: fp32 / bf16 / fp16, widened to fp32.
+    Returns fixed-capacity tensors (bboxes (bs, max_num, 9) f32, scores (bs, max_num) f32, labels (bs, max_num) i64,
+    num (bs,) i32): sample i's detections are the first num[i] rows, in the order (score descending, flat index
+    ascending) -- torch.topk leaves the order of equal scores unspecified; this kernel takes the lower flat index
+    first.  Rows past num are zero.  ``score_threshold`` follows the reference's loop, including its quirks (0.0
+    applies no mask); ``z_shift`` applies BEVFormerHead.get_bboxes' z -= h / 2."""
+    if post_center_range is None:
+        raise NotImplementedError("Need to reorganize output as a batch, only support post_center_range is not None "
+                                  "for now!")
+    for name, t in (("cls_scores", cls_scores), ("bbox_preds", bbox_preds)):
+        _need_cuda(t, name)
+        if t.dtype not in _DT:
+            raise RuntimeError(f"nms_free_decode: {name} must be float32, bfloat16 or float16")
+    if cls_scores.dim() != 3 or bbox_preds.dim() != 3 or bbox_preds.shape[:2] != cls_scores.shape[:2]:
+        raise RuntimeError(f"nms_free_decode: shapes {tuple(cls_scores.shape)} / {tuple(bbox_preds.shape)}; need "
+                           "(bs, nq, ncls) / (bs, nq, 10)")
+    bs, nq, ncls = cls_scores.shape
+    if bbox_preds.shape[2] != 10:
+        raise RuntimeError("nms_free_decode: code_size must be 10")
+    max_num = int(max_num)
+    if not 1 <= max_num <= nq * ncls:
+        raise RuntimeError(f"nms_free_decode: max_num {max_num} must lie in [1, nq * ncls = {nq * ncls}]")
+    lib = _lib.load()
+    if lib.bevf_nms_free_decode_smem_bytes(nq, ncls, max_num) > 200 * 1024:
+        raise RuntimeError(f"nms_free_decode: nq * ncls = {nq * ncls} is too large for the shared-memory top-k")
+    import ctypes
+    import numpy as np
+    pcr = (ctypes.c_float * 6)(*np.asarray(post_center_range, dtype=np.float32).reshape(6).tolist())
+    dev = cls_scores.device
+    bboxes = torch.empty((bs, max_num, 9), device=dev, dtype=torch.float32)
+    scores = torch.empty((bs, max_num), device=dev, dtype=torch.float32)
+    labels = torch.empty((bs, max_num), device=dev, dtype=torch.int64)
+    num = torch.empty((bs,), device=dev, dtype=torch.int32)
+    has_thr = score_threshold is not None and bool(score_threshold)
+    with torch.cuda.device(dev):
+        st = lib.bevf_nms_free_decode(cls_scores.data_ptr(), _DT[cls_scores.dtype], bbox_preds.data_ptr(),
+                                      _DT[bbox_preds.dtype], bs, nq, ncls, 10, max_num, ctypes.cast(pcr, ctypes.c_void_p),
+                                      int(has_thr), float(score_threshold) if has_thr else 0.0, int(bool(z_shift)),
+                                      bboxes.data_ptr(), scores.data_ptr(), labels.data_ptr(), num.data_ptr(),
+                                      _stream_ptr(cls_scores))
+    _lib.check(st, lib)
+    return bboxes, scores, labels, num

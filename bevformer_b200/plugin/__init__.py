@@ -9,10 +9,13 @@ from .registry import (ATTENTION, FEEDFORWARD_NETWORK, TRANSFORMER_LAYER, TRANSF
 from .spatial_cross_attention import MSDeformableAttention3D, ScaPlan, SpatialCrossAttention
 from .temporal_self_attention import TemporalSelfAttention
 from .temporal import BEVStream, obtain_history_bev
+from .head import BEVFormerHead, BEVFormerHead_GroupDETR, LearnedPositionalEncoding, NMSFreeCoder
+from .registry import BBOX_CODERS, HEADS, POSITIONAL_ENCODING
 from .transformer import (PerceptionTransformer, PerceptionTransformerBEVEncoder, PerceptionTransformerV2,
                           ResNetFusion)
 
-__all__ = ["PerceptionTransformerV2", "ResNetFusion", "BEVStream", "obtain_history_bev", "PerceptionTransformer", "PerceptionTransformerBEVEncoder", "CustomMSDeformableAttention", "DetectionTransformerDecoder",
+__all__ = ["BEVFormerHead", "BEVFormerHead_GroupDETR", "LearnedPositionalEncoding", "NMSFreeCoder", "HEADS",
+           "BBOX_CODERS", "POSITIONAL_ENCODING", "PerceptionTransformerV2", "ResNetFusion", "BEVStream", "obtain_history_bev", "PerceptionTransformer", "PerceptionTransformerBEVEncoder", "CustomMSDeformableAttention", "DetectionTransformerDecoder",
            "DetrTransformerDecoderLayer", "GroupMultiheadAttention", "MultiheadAttention", "inverse_sigmoid", "BEVFormerEncoder", "BEVFormerLayer", "MyCustomBaseTransformerLayer", "FFN",
            "SpatialCrossAttention", "MSDeformableAttention3D", "TemporalSelfAttention", "ScaPlan",
            "ATTENTION", "FEEDFORWARD_NETWORK", "TRANSFORMER_LAYER", "TRANSFORMER_LAYER_SEQUENCE",

@@ -71,6 +71,27 @@ except Exception:  # noqa: BLE001
         TRANSFORMER = Registry("Transformer")
 
 
+# BEVFormerHead / NMSFreeCoder / LearnedPositionalEncoding register where the reference's classes do: mmdet's HEADS
+# (dense_heads/bevformer_head.py:16), mmdet's BBOX_CODERS (core/bbox/coders/nms_free_coder.py:9) and mmcv's
+# POSITIONAL_ENCODING (mmdet 2.14 models/utils/positional_encoding.py)
+def _registry(import_name, attr, name):
+    try:  # pragma: no cover - mmdet / mmcv are absent from the build image
+        if not HAVE_MMCV:
+            raise ImportError(import_name)
+        import importlib
+        return getattr(importlib.import_module(import_name), attr)
+    except Exception:  # noqa: BLE001
+        if HAVE_MMCV:
+            from mmcv.utils import Registry as _MmcvRegistry
+            return _MmcvRegistry(name)
+        return Registry(name)
+
+
+HEADS = _registry("mmdet.models.builder", "HEADS", "head")
+BBOX_CODERS = _registry("mmdet.core.bbox.builder", "BBOX_CODERS", "bbox_coder")
+POSITIONAL_ENCODING = _registry("mmcv.cnn.bricks.registry", "POSITIONAL_ENCODING", "position encoding")
+
+
 def _register(registry, cls, name=None):
     """Register without tripping over a name mmcv (or an earlier import) already holds."""
     try:

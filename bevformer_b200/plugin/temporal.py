@@ -30,6 +30,36 @@ def _on_device(can_bus) -> bool:
     return torch.is_tensor(can_bus) and can_bus.is_cuda
 
 
+# a detection frame's outputs, in the order the captured mode keeps its static buffers (the BEV first)
+_DET_KEYS = ("bev_embed", "all_cls_scores", "all_bbox_preds", "bboxes", "scores", "labels", "num")
+
+
+class _DetFrame:
+    """A frame through a detection head (plugin.head.BEVFormerHead): ``head.forward`` in eval mode -- the head
+    builds its own BEV queries, positional encoding and object queries -- then the coder's ``decode_device``."""
+
+    def __init__(self, head):
+        self.head = head
+
+    def __call__(self, mlvl_feats, prev_bev=None, img_metas=None, grid_length=None, bev_pos=None, **device_kwargs):
+        was_training = self.head.training
+        self.head.eval()
+        try:
+            out = self.head(mlvl_feats, img_metas, prev_bev=prev_bev, **device_kwargs)
+        finally:
+            self.head.train(was_training)
+        dec = self.head.bbox_coder.decode_device(out)
+        return {k: out[k] if k in out else dec[k] for k in _DET_KEYS}
+
+
+def _bev_of(res):
+    """The BEV of a frame's result: the tensor itself, a transformer 4-tuple's first entry, a detection dict's
+    ``bev_embed``."""
+    if torch.is_tensor(res):
+        return res
+    return res["bev_embed"] if isinstance(res, dict) else res[0]
+
+
 def obtain_history_bev(transformer, feats_queue: Sequence[torch.Tensor], img_metas_list, bev_queries,
                        bev_h: int, bev_w: int, bev_pos, grid_length=(0.512, 0.512), can_bus=None,
                        lidar2img=None) -> Optional[torch.Tensor]:
@@ -89,6 +119,10 @@ class BEVStream:
     ``reg_branches`` / ``cls_branches``) and returns its 4-tuple (bev_embed (Nq, bs, C), inter_states,
     init_reference_out, inter_references_out); bev_embed becomes the next frame's prev_bev.  Without it a frame is
     ``get_bev_features`` and returns the BEV alone.
+    With ``head`` (plugin.head.BEVFormerHead, whose transformer is this stream's) a frame is ``head.forward`` plus
+    its coder's ``decode_device`` and returns ``dict(bev_embed, all_cls_scores, all_bbox_preds, bboxes, scores, labels,
+    num)`` (the decode's fixed-capacity tensors: no host synchronisation); ``bev_queries`` / ``bev_pos`` /
+    ``grid_length`` are then the head's own and the arguments of those names are not read.
     ``prev_frame_info["scene_token"]`` and ``["prev_bev"]`` are shared by the three; do not mix the host path with
     the other two inside one scene (each keeps its own previous position / angle)."""
 
@@ -108,7 +142,7 @@ class BEVStream:
     @torch.no_grad()
     def step(self, mlvl_feats: Optional[List[torch.Tensor]], img_metas: List[dict], bev_queries=None, bev_h: int = None,
              bev_w: int = None, bev_pos=None, grid_length=(0.512, 0.512), can_bus=None, lidar2img=None,
-             object_query_embed=None, reg_branches=None, cls_branches=None):
+             object_query_embed=None, reg_branches=None, cls_branches=None, head=None):
         """One frame: mlvl_feats per level (bs, num_cams, C, h, w), img_metas one dict per sample with
         ABSOLUTE ``can_bus`` and a ``scene_token``.  Returns this frame's BEV (bs, Nq, C), which also becomes
         the next frame's ``prev_bev``.  The caller's metas are not modified (the reference edits them in
@@ -124,7 +158,10 @@ class BEVStream:
         (in captured mode, what ``capture`` was given decides, and these are ignored)."""
         if self._graphs is not None:
             return self._step_captured(mlvl_feats, img_metas, can_bus, lidar2img)
-        head = None if object_query_embed is None else (object_query_embed, reg_branches, cls_branches)
+        if head is not None:
+            head = _DetFrame(head)
+        elif object_query_embed is not None:
+            head = (object_query_embed, reg_branches, cls_branches)
         info = self.prev_frame_info
         if img_metas[0].get("scene_token") != info["scene_token"]:
             info["prev_bev"] = None                                  # :243-245
@@ -134,7 +171,7 @@ class BEVStream:
         if _on_device(can_bus):
             res = self._frame(mlvl_feats, img_metas, bev_queries, bev_h, bev_w, bev_pos, grid_length, can_bus,
                               lidar2img, info["prev_bev"], head)
-            info["prev_bev"] = res if head is None else res[0]
+            info["prev_bev"] = _bev_of(res)
             return res
         metas = [dict(m) for m in img_metas]
         can_bus = np.array(metas[0]["can_bus"], dtype=np.float64, copy=True)
@@ -153,15 +190,17 @@ class BEVStream:
                             bev_pos=bev_pos, prev_bev=info["prev_bev"], img_metas=metas)
         finally:
             self.transformer.train(was_training)
-        bev = res if head is None else res[0]
+        bev = _bev_of(res)
         info["prev_pos"], info["prev_angle"], info["prev_bev"] = tmp_pos, tmp_angle, bev    # :266-268
         return res
 
     def _run(self, head, mlvl_feats, bev_queries, bev_h, bev_w, **kwargs):
         """get_bev_features, or with ``head`` = (object_query_embed, reg_branches, cls_branches) the whole
-        transformer."""
+        transformer; with a ``_DetFrame`` the detection frame."""
         if head is None:
             return self.transformer.get_bev_features(mlvl_feats, bev_queries, bev_h, bev_w, **kwargs)
+        if isinstance(head, _DetFrame):
+            return head(mlvl_feats, **kwargs)
         oq, reg, cls = head
         return self.transformer(mlvl_feats, bev_queries, oq, bev_h, bev_w, reg_branches=reg, cls_branches=cls,
                                 **kwargs)
@@ -185,9 +224,9 @@ class BEVStream:
 
     # ---- captured mode ------------------------------------------------------------------------------------------
     @torch.no_grad()
-    def capture(self, mlvl_feats: List[torch.Tensor], img_metas: List[dict], bev_queries, bev_h: int, bev_w: int,
-                bev_pos, grid_length=(0.512, 0.512), *, can_bus, lidar2img, object_query_embed=None,
-                reg_branches=None, cls_branches=None) -> dict:
+    def capture(self, mlvl_feats: List[torch.Tensor], img_metas: List[dict], bev_queries=None, bev_h: int = None,
+                bev_w: int = None, bev_pos=None, grid_length=(0.512, 0.512), *, can_bus, lidar2img,
+                object_query_embed=None, reg_branches=None, cls_branches=None, head=None) -> dict:
         """Record the device path for these shapes as two CUDA graphs -- first frame of a scene (no history: the
         temporal self-attention stacks the query with itself) and continuation (prev_bev = the previous output,
         rotated) -- over static input buffers, returned (and kept as ``self.static``): ``{"feats": [per level],
@@ -200,7 +239,8 @@ class BEVStream:
         device-path frame with it and ``encoder.check_plan()``, and capture again if that raises.
 
         With ``object_query_embed`` the graphs record the whole transformer (encoder and decoder; the embedding and
-        the branches are read in place by every replay) and ``step`` returns the static 4-tuple of output buffers."""
+        the branches are read in place by every replay) and ``step`` returns the static 4-tuple of output buffers; with
+        ``head`` the graphs record the detection frame and ``step`` returns its dict of static output buffers."""
         if not (_on_device(can_bus) and _on_device(lidar2img)):
             raise RuntimeError("BEVStream.capture: can_bus and lidar2img must be CUDA tensors (the device path)")
         self._graphs = None
@@ -209,7 +249,8 @@ class BEVStream:
                            lidar2img=lidar2img.detach().to(torch.float32).clone())
         self._cap = dict(img_metas=[dict(img_shape=img_metas[0]["img_shape"]) for _ in img_metas],
                          bev_queries=bev_queries, bev_h=bev_h, bev_w=bev_w, bev_pos=bev_pos, grid_length=grid_length,
-                         head=None if object_query_embed is None else (object_query_embed, reg_branches, cls_branches))
+                         head=_DetFrame(head) if head is not None else
+                         None if object_query_embed is None else (object_query_embed, reg_branches, cls_branches))
         self._record()
         return self.static
 
@@ -221,7 +262,9 @@ class BEVStream:
         def frame(prev):                                   # the frame's outputs as a tuple, bev first
             res = self._frame(st["feats"], c["img_metas"], c["bev_queries"], c["bev_h"], c["bev_w"], c["bev_pos"],
                               c["grid_length"], st["can_bus"], st["lidar2img"], prev, c["head"])
-            return (res,) if c["head"] is None else tuple(res)
+            if c["head"] is None:
+                return (res,)
+            return tuple(res[k] for k in _DET_KEYS) if isinstance(res, dict) else tuple(res)
 
         cur = torch.cuda.current_stream(dev)
         side = torch.cuda.Stream(dev)
@@ -237,7 +280,11 @@ class BEVStream:
                 for o, r in zip(outs, frame(None if kind == "first" else outs[0])):
                     o.copy_(r)
             graphs[kind], pool = g, g.pool()
-        self._graphs, self._out = graphs, (outs[0] if c["head"] is None else outs)
+        if c["head"] is None:
+            out = outs[0]
+        else:
+            out = dict(zip(_DET_KEYS, outs)) if isinstance(c["head"], _DetFrame) else outs
+        self._graphs, self._out = graphs, out
         self.reset()
 
     def _step_captured(self, mlvl_feats, img_metas, can_bus, lidar2img):
@@ -252,5 +299,5 @@ class BEVStream:
         first = token != info["scene_token"] or info["prev_bev"] is None or not self.video_test_mode
         info["scene_token"] = token
         self._graphs["first" if first else "cont"].replay()
-        info["prev_bev"] = self._out if self._cap["head"] is None else self._out[0]
+        info["prev_bev"] = _bev_of(self._out)
         return self._out

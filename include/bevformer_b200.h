@@ -40,7 +40,7 @@
 extern "C" {
 #endif
 
-#define BEVF_ABI_VERSION 2
+#define BEVF_ABI_VERSION 3
 
 #if defined(__GNUC__)
 #define BEVF_API __attribute__((visibility("default")))
@@ -690,6 +690,49 @@ BEVF_API int bevf_ego_motion(const double *can_bus, void *state, int mode, float
                              double grid_w, double center_x, double center_y, int use_shift, void *stream);
 BEVF_API int bevf_rotate_bev(const void *prev, int in_dtype, int64_t stride_q, int64_t stride_b, const float *rot,
                              void *out, int out_dtype, int bs, int bev_h, int bev_w, int C, void *stream);
+
+/*
+ * Detection head (BEVFormerHead.forward after the transformer, dense_heads/bevformer_head.py:171-203), inference only:
+ * per decoder level l the classification branch (Linear-LayerNorm-ReLU x 2, Linear -> ncls) and the regression branch
+ * (Linear-ReLU x 2, Linear -> 10) on the level's decoder states, then on the regression output
+ *   out[c] = sigmoid(tmp[c] + inverse_sigmoid(ref[c'])) * (pc_range[c' + 3] - pc_range[c']) + pc_range[c'],
+ *   (c, c') in {(0, 0), (1, 1), (4, 2)}, inverse_sigmoid with eps 1e-5, evaluated in fp32 and rounded once.
+ * One launch, one CTA per (level, branch, 64-row tile); the hidden activations stay in shared memory.
+ *   x          decoder states (L, nq, bs, C = 256) in `dtype` (bf16 | f16): element (l, q, b, c) at
+ *              x[l * stride_l + q * stride_q + b * stride_b + c]; strides multiples of 8
+ *   ref0       (bs, nq, 3) initial reference points; refs (L, bs, nq, 3) the decoder's, level l > 0 reads refs[l - 1];
+ *              both in ref_dtype (f32 | bf16 | f16)
+ *   params     HOST array of L * 16 device pointers, per level: cls W0 b0 gamma0 beta0 W1 b1 gamma1 beta1 W2 b2, then
+ *              reg W0 b0 W1 b1 W2 b2; weights row-major (out, 256); all in param_dtype (`dtype` or f32: fp32 weights
+ *              and Linear biases are rounded to `dtype`, as autocast's Linear rounds them; LayerNorm's in fp32).  Copied into the kernel's parameters at the call, so a
+ *              captured launch keeps reading the same parameter tensors.
+ *   cls_out    (L, bs, nq, ncls) and box_out (L, bs, nq, 10) in `dtype`
+ *   1 <= L <= 8, ncls <= 16, code_size == 10; ln_eps the LayerNorms' eps; pc_range HOST array of 6 doubles.
+ */
+BEVF_API int bevf_det_branches_forward(const void *x, int64_t stride_l, int64_t stride_q, int64_t stride_b, int dtype,
+                                       const void *ref0, const void *refs, int ref_dtype, const void *const *params,
+                                       int param_dtype, void *cls_out, void *box_out, int L, int bs, int nq, int C,
+                                       int ncls, int code_size, float ln_eps, const double *pc_range, void *stream);
+
+/*
+ * NMSFreeCoder.decode (core/bbox/coders/nms_free_coder.py:40-121) for a batch, one CTA per sample, no host
+ * synchronisation.  cls (bs, nq, ncls) logits and box (bs, nq, 10) normalised boxes, contiguous, any dtype code
+ * (widened to fp32).  scores = 1 / (1 + expf(-x)) in IEEE fp32 (torch.sigmoid's arithmetic, subnormal results
+ * included); the max_num largest of the nq * ncls scores are
+ * selected and ordered by (score descending, flat index ascending) -- a tie rule torch.topk leaves unspecified;
+ * label = idx % ncls, box = denormalize_bbox(box[idx / ncls]) = (cx, cy, cz, exp w, exp l, exp h,
+ * atan2(sin, cos), vx, vy).  With has_threshold (a threshold that is given and non-zero) the reference's decay loop
+ * picks the mask: score > t, else score >= t * 0.9^i (t * 0.9^i in double, compared in fp32) for the first i
+ * the top score passes, else (t * 0.9^i < 0.01) score > -1.  Kept: centre within post_center_range (HOST float[6],
+ * inclusive) and the threshold mask.  Outputs, in candidate order, compacted: bboxes (bs, max_num, 9) f32,
+ * scores (bs, max_num) f32, labels (bs, max_num) i64, num (bs) i32; slots past num are zero.  z_shift: z -= h / 2
+ * (BEVFormerHead.get_bboxes).  max_num <= nq * ncls and bevf_nms_free_decode_smem_bytes(...) <= 200 KiB.
+ */
+BEVF_API int bevf_nms_free_decode(const void *cls, int cls_dtype, const void *box, int box_dtype, int bs, int nq,
+                                  int ncls, int code_size, int max_num, const float *post_center_range,
+                                  int has_threshold, double score_threshold, int z_shift, float *bboxes,
+                                  float *scores, int64_t *labels, int *num, void *stream);
+BEVF_API int64_t bevf_nms_free_decode_smem_bytes(int nq, int ncls, int max_num);
 
 #ifdef __cplusplus
 }

@@ -1,0 +1,2 @@
+# Same import surface as the reference package of this path (the implementation lives in bevformer_b200/plugin/head.py).
+from .bevformer_head import BEVFormerHead, BEVFormerHead_GroupDETR
