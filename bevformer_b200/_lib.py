@@ -132,6 +132,13 @@ SIGNATURES = {
     "bevf_nms_free_decode": (c_int, [c_void_p, c_int, c_void_p, c_int] + [c_int] * 5
                              + [c_void_p, c_int, ctypes.c_double, c_int] + [c_void_p] * 5),
     "bevf_nms_free_decode_smem_bytes": (c_int64, [c_int, c_int, c_int]),
+    "bevf_det_match_cost": (c_int, [c_void_p, c_int, c_void_p, c_int] + [c_void_p] * 4 + [c_int] * 6
+                            + [ctypes.c_float] * 5 + [c_void_p]),
+    "bevf_det_match_cost_smem_bytes": (c_int64, [c_int, c_int]),
+    "bevf_det_loss_forward": (c_int, [c_void_p, c_int, c_void_p, c_int] + [c_void_p] * 8 + [c_int] * 7
+                              + [ctypes.c_float] * 5 + [c_void_p]),
+    "bevf_det_loss_backward": (c_int, [c_void_p, c_int, c_void_p, c_int] + [c_void_p] * 10 + [c_int] * 7
+                               + [ctypes.c_float] * 5 + [c_void_p]),
 }
 
 

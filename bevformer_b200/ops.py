@@ -1677,3 +1677,132 @@ def nms_free_decode(cls_scores, bbox_preds, max_num, post_center_range, score_th
                                       _stream_ptr(cls_scores))
     _lib.check(st, lib)
     return bboxes, scores, labels, num
+
+
+# ---------------------------------------------------------------------------------------------------
+# Detection loss (csrc/det_loss.cu): the matching cost of every (layer, sample) in one launch, and the focal /
+# L1 / smooth-L1 losses of every (layer, group) slot with their gradient.  The assignment between them is the host's.
+# ---------------------------------------------------------------------------------------------------
+DET_REG = {"l1": 0, "smooth_l1": 1}
+
+
+def _det_preds(cls_scores, bbox_preds, who):
+    for name, t in (("cls_scores", cls_scores), ("bbox_preds", bbox_preds)):
+        _need_cuda(t, name)
+        if t.dtype not in _DT:
+            raise RuntimeError(f"{who}: {name} must be float32, bfloat16 or float16")
+    if (cls_scores.dim() != 4 or bbox_preds.dim() != 4 or bbox_preds.shape[:3] != cls_scores.shape[:3]
+            or bbox_preds.shape[3] != 10):
+        raise RuntimeError(f"{who}: shapes {tuple(cls_scores.shape)} / {tuple(bbox_preds.shape)}; need "
+                           "(L, bs, nq, ncls) / (L, bs, nq, 10)")
+    return cls_scores.shape
+
+
+def _det_gt(gt, gt_labels, n_gt, bs, device, who):
+    G = gt.shape[1]
+    if (gt.dtype != torch.float32 or tuple(gt.shape) != (bs, G, 9) or gt_labels.dtype != torch.int64
+            or tuple(gt_labels.shape) != (bs, G) or n_gt.dtype != torch.int32 or tuple(n_gt.shape) != (bs,)):
+        raise RuntimeError(f"{who}: ground truth must be gt (bs, G, 9) float32, gt_labels (bs, G) int64 and "
+                           f"n_gt (bs,) int32; got {tuple(gt.shape)} {gt.dtype}, {tuple(gt_labels.shape)} "
+                           f"{gt_labels.dtype}, {tuple(n_gt.shape)} {n_gt.dtype}")
+    for name, t in (("gt", gt), ("gt_labels", gt_labels), ("n_gt", n_gt)):
+        _need_cuda(t, name)
+        if t.device != device:
+            raise RuntimeError(f"{who}: {name} must be on the predictions' device ({device})")
+    return G
+
+
+def det_match_cost(cls_scores, bbox_preds, gt, gt_labels, n_gt, reg_kind, cls_weight, reg_weight, alpha=0.25,
+                   gamma=2.0, eps=1e-12):
+    """HungarianAssigner3D's cost (hungarian_assigner_3d.py:106-116) for every decoder layer and sample in one launch.
+
+    cls_scores (L, bs, nq, ncls) / bbox_preds (L, bs, nq, 10): fp32, bf16 or fp16.  gt (bs, G, 9) f32 gravity-centred
+    boxes, gt_labels (bs, G) i64, n_gt (bs,) i32, all on the device; reg_kind 'l1' (BBox3DL1Cost) or 'smooth_l1'
+    (SmoothL1Cost).  Returns the fp32 cost (L * bs, nq, G): row l * bs + b; columns past n_gt[b] are zero."""
+    L, bs, nq, ncls = _det_preds(cls_scores, bbox_preds, "det_match_cost")
+    G = _det_gt(gt, gt_labels, n_gt, bs, cls_scores.device, "det_match_cost")
+    if reg_kind not in DET_REG:
+        raise RuntimeError(f"det_match_cost: reg_kind must be one of {sorted(DET_REG)}")
+    if G == 0:
+        raise RuntimeError("det_match_cost: no ground-truth column (G = 0)")
+    if not 1 <= ncls <= 64:
+        raise RuntimeError(f"det_match_cost: {ncls} classes; the kernel takes 1 to 64")
+    lib = _lib.load()
+    if lib.bevf_det_match_cost_smem_bytes(ncls, G) > 200 * 1024:
+        raise RuntimeError(f"det_match_cost: {G} ground-truth boxes per sample is more than the kernel's tile holds")
+    cost = torch.empty((L * bs, nq, G), device=cls_scores.device, dtype=torch.float32)
+    with torch.cuda.device(cls_scores.device):
+        st = lib.bevf_det_match_cost(cls_scores.data_ptr(), _DT[cls_scores.dtype], bbox_preds.data_ptr(),
+                                     _DT[bbox_preds.dtype], gt.data_ptr(), gt_labels.data_ptr(), n_gt.data_ptr(),
+                                     cost.data_ptr(), L * bs, bs, nq, ncls, G, DET_REG[reg_kind], float(cls_weight),
+                                     float(reg_weight), float(alpha), float(gamma), float(eps),
+                                     _stream_ptr(cls_scores))
+    _lib.check(st, lib)
+    return cost
+
+
+class DetLoss(Function):
+    """BEVFormerHead.loss_single after the assignment, for every (layer, group) slot in one launch each way.
+
+    apply(cls_scores, bbox_preds, assign, gt, gt_labels, n_gt, code_weights, avg, cfg) -> (L * groups, 2) fp32
+    [loss_cls, loss_bbox] per slot s = l * groups + group, nan_to_num applied.
+      cls_scores / bbox_preds  (L, bs, nq, ncls) / (L, bs, nq, 10), fp32 / bf16 / fp16; their gradients come back in
+                               their own dtype
+      assign                   (L * bs, nq) int32 ground-truth index or -1
+      gt / gt_labels / n_gt    as det_match_cost; code_weights (10,) f32; avg (L * groups, 2) f32 avg factors
+                               (cls, regression) before max(., 1), in device memory
+      cfg                      dict(groups, reg_kind, cls_loss_weight, bbox_loss_weight, alpha, gamma, beta)
+    Both directions are sums in a fixed order: the results repeat bit for bit."""
+
+    @staticmethod
+    def _args(cls_scores, bbox_preds, assign, gt, gt_labels, n_gt, code_weights, avg, cfg):
+        L, bs, nq, ncls = _det_preds(cls_scores, bbox_preds, "DetLoss")
+        G = _det_gt(gt, gt_labels, n_gt, bs, cls_scores.device, "DetLoss")
+        groups = int(cfg["groups"])
+        if groups < 1 or nq % groups:
+            raise RuntimeError(f"DetLoss: {nq} queries do not split into {groups} groups")
+        for name, t, dt, shp in (("assign", assign, torch.int32, (L * bs, nq)),
+                                 ("code_weights", code_weights, torch.float32, (10,)),
+                                 ("avg", avg, torch.float32, (L * groups, 2))):
+            _need_cuda(t, name)
+            if t.dtype != dt or tuple(t.shape) != shp or t.device != cls_scores.device:
+                raise RuntimeError(f"DetLoss: {name} must be {dt} of shape {shp} on {cls_scores.device}, got "
+                                   f"{t.dtype} {tuple(t.shape)} on {t.device}")
+        if cfg["reg_kind"] not in DET_REG:
+            raise RuntimeError(f"DetLoss: reg_kind must be one of {sorted(DET_REG)}")
+        head = [cls_scores.data_ptr(), _DT[cls_scores.dtype], bbox_preds.data_ptr(), _DT[bbox_preds.dtype],
+                assign.data_ptr(), gt.data_ptr(), gt_labels.data_ptr(), n_gt.data_ptr(), code_weights.data_ptr(),
+                avg.data_ptr()]
+        tail = [L, bs, nq, groups, ncls, G, DET_REG[cfg["reg_kind"]], float(cfg["cls_loss_weight"]),
+                float(cfg["bbox_loss_weight"]), float(cfg["alpha"]), float(cfg["gamma"]), float(cfg.get("beta", 1.0)),
+                _stream_ptr(cls_scores)]
+        return head, tail, L * groups
+
+    @staticmethod
+    def forward(ctx, cls_scores, bbox_preds, assign, gt, gt_labels, n_gt, code_weights, avg, cfg):
+        cls_scores, bbox_preds = cls_scores.contiguous(), bbox_preds.contiguous()
+        head, tail, S = DetLoss._args(cls_scores, bbox_preds, assign, gt, gt_labels, n_gt, code_weights, avg, cfg)
+        out = torch.empty((2, S, 2), device=cls_scores.device, dtype=torch.float32)
+        lib = _lib.load()
+        with torch.cuda.device(cls_scores.device):
+            st = lib.bevf_det_loss_forward(*head, out[0].data_ptr(), out[1].data_ptr(), *tail)
+        _lib.check(st, lib)
+        ctx.save_for_backward(cls_scores, bbox_preds, assign, gt, gt_labels, n_gt, code_weights, avg, out[1])
+        ctx.cfg = cfg
+        return out[0]
+
+    @staticmethod
+    @once_differentiable
+    def backward(ctx, grad_loss):
+        cls_scores, bbox_preds, assign, gt, gt_labels, n_gt, code_weights, avg, loss_raw = ctx.saved_tensors
+        head, tail, S = DetLoss._args(cls_scores, bbox_preds, assign, gt, gt_labels, n_gt, code_weights, avg,
+                                      ctx.cfg)
+        grad_loss = grad_loss.to(torch.float32).contiguous()
+        grad_cls = torch.empty_like(cls_scores)
+        grad_box = torch.empty_like(bbox_preds)
+        lib = _lib.load()
+        with torch.cuda.device(cls_scores.device):
+            st = lib.bevf_det_loss_backward(*head, loss_raw.data_ptr(), grad_loss.data_ptr(), grad_cls.data_ptr(),
+                                            grad_box.data_ptr(), *tail)
+        _lib.check(st, lib)
+        return grad_cls, grad_box, None, None, None, None, None, None, None

@@ -2,8 +2,7 @@
 
 Drop-ins for the reference classes of the same names (projects/mmdet3d_plugin/bevformer/dense_heads/bevformer_head.py,
 projects/mmdet3d_plugin/core/bbox/coders/nms_free_coder.py, mmdet 2.14's LearnedPositionalEncoding): same constructor
-arguments, parameter names and return values, for inference.  The training loss (matching, focal / L1 losses,
-``get_targets``) is not part of this module.
+arguments, parameter names and return values, and ``loss`` with the reference's signature and loss dict.
 
 What changes underneath:
   * the classification / regression branches of every decoder level and the box-centre arithmetic after them run as
@@ -11,7 +10,12 @@ What changes underneath:
     gradient run the head's own ``nn.Sequential`` branches and the reference's arithmetic in torch;
   * the coder's sigmoid / top-k / denormalisation / score threshold / centre-range filter is one kernel per batch
     (``ops.nms_free_decode``) with fixed-capacity outputs and no host synchronisation (``decode_device``);
-    ``decode`` and ``get_bboxes`` synchronise once to slice the detections.
+    ``decode`` and ``get_bboxes`` synchronise once to slice the detections;
+  * ``loss`` builds the matching cost of every decoder layer, group and sample in one kernel
+    (``ops.det_match_cost``), copies it to the host once -- the call's only synchronisation -- and runs the
+    reference's own ``scipy.optimize.linear_sum_assignment`` on each (layer, group, sample) slice; targets, focal and
+    L1 / smooth-L1 losses and their gradients are one kernel each way (``ops.DetLoss``), with the avg factors kept
+    in device memory.
 """
 from __future__ import annotations
 
@@ -96,10 +100,114 @@ class NMSFreeCoder:
 
 
 def _loss_cfg(cfg):
-    """A loss config kept for its settings: the head reads ``use_sigmoid`` only (FocalLoss's default is True)."""
+    """A loss config kept for its settings, with mmdet 2.14's defaults: ``use_sigmoid`` (FocalLoss: True),
+    ``loss_weight`` 1, FocalLoss's ``gamma`` 2 / ``alpha`` 0.25, SmoothL1Loss's ``beta`` 1."""
     cfg = dict(cfg or {})
     cfg.setdefault("use_sigmoid", cfg.get("type") == "FocalLoss")
+    cfg.setdefault("loss_weight", 1.0)
+    if cfg.get("type") == "FocalLoss":
+        cfg.setdefault("gamma", 2.0)
+        cfg.setdefault("alpha", 0.25)
+    if cfg.get("type") == "SmoothL1Loss":
+        cfg.setdefault("beta", 1.0)
     return types.SimpleNamespace(**cfg)
+
+
+_REG_COSTS = {"BBox3DL1Cost": "l1", "SmoothL1Cost": "smooth_l1"}
+_REG_LOSSES = {"L1Loss": "l1", "SmoothL1Loss": "smooth_l1"}
+
+
+def _loss_settings(head):
+    """The assigner's and losses' settings ``loss`` runs with (``train_cfg['assigner']``, ``loss_cls``,
+    ``loss_bbox``), checked as mmdet 2.14's DETRHead checks them: the cost and loss weights must agree.  Only the
+    costs and losses the shipped configs use are implemented; anything else raises."""
+    assigner = (head.train_cfg or {}).get("assigner")
+    if assigner is None:
+        raise RuntimeError(f"{type(head).__name__}.loss: train_cfg has no 'assigner' (the detector passes "
+                           "train_cfg['pts'] of the config, which holds HungarianAssigner3D's settings)")
+    if assigner.get("type", "HungarianAssigner3D") != "HungarianAssigner3D":
+        raise NotImplementedError(f"loss: assigner {assigner.get('type')!r}; only HungarianAssigner3D is implemented")
+    cls_cost = dict(assigner.get("cls_cost", dict(type="ClassificationCost", weight=1.0)))
+    reg_cost = dict(assigner.get("reg_cost", dict(type="BBoxL1Cost", weight=1.0)))
+    if cls_cost.get("type") != "FocalLossCost":
+        raise NotImplementedError(f"loss: cls_cost {cls_cost.get('type')!r}; only FocalLossCost is implemented")
+    if reg_cost.get("type") not in _REG_COSTS:
+        raise NotImplementedError(f"loss: reg_cost {reg_cost.get('type')!r}; only {sorted(_REG_COSTS)} are "
+                                  "implemented")
+    lc, lb = head.loss_cls, head.loss_bbox
+    if getattr(lc, "type", None) != "FocalLoss" or not lc.use_sigmoid:
+        raise NotImplementedError(f"loss: loss_cls {getattr(lc, 'type', None)!r}; only FocalLoss(use_sigmoid=True) "
+                                  "is implemented")
+    if getattr(lb, "type", None) not in _REG_LOSSES:
+        raise NotImplementedError(f"loss: loss_bbox {getattr(lb, 'type', None)!r}; only {sorted(_REG_LOSSES)} are "
+                                  "implemented")
+    for name, loss in (("loss_cls", lc), ("loss_bbox", lb)):
+        if getattr(loss, "reduction", "mean") != "mean":
+            raise NotImplementedError(f"loss: {name} with reduction={loss.reduction!r}; only 'mean' is implemented")
+    cls_w, reg_w = cls_cost.get("weight", 1.0), reg_cost.get("weight", 1.0)
+    if lc.loss_weight != cls_w:
+        raise ValueError(f"loss: the classification weight for loss and matcher should be exactly the same "
+                         f"(loss_cls.loss_weight {lc.loss_weight}, cls_cost.weight {cls_w})")
+    if lb.loss_weight != reg_w:
+        raise ValueError(f"loss: the regression weight for loss and matcher should be exactly the same "
+                         f"(loss_bbox.loss_weight {lb.loss_weight}, reg_cost.weight {reg_w})")
+    return dict(cost_reg_kind=_REG_COSTS[reg_cost["type"]], cls_cost_weight=float(cls_w),
+                reg_cost_weight=float(reg_w), cost_alpha=float(cls_cost.get("alpha", 0.25)),
+                cost_gamma=float(cls_cost.get("gamma", 2)), cost_eps=float(cls_cost.get("eps", 1e-12)),
+                reg_kind=_REG_LOSSES[lb.type], cls_loss_weight=float(lc.loss_weight),
+                bbox_loss_weight=float(lb.loss_weight), alpha=float(lc.alpha), gamma=float(lc.gamma),
+                beta=float(getattr(lb, "beta", 1.0)))
+
+
+def gravity_center_boxes(boxes):
+    """``cat(gravity_center, tensor[:, 3:])`` (bevformer_head.py:441-443) as an (n, 9) float32 tensor.  Takes an
+    object with ``gravity_center`` and ``tensor`` (mmdet3d's LiDARInstance3DBoxes) or a plain (n, 9) tensor in that
+    class's layout (x, y, z_bottom, w, l, h, yaw, vx, vy), whose gravity centre is z + h / 2."""
+    if hasattr(boxes, "gravity_center") and hasattr(boxes, "tensor"):
+        out = torch.cat((boxes.gravity_center, boxes.tensor[:, 3:]), dim=1)
+    elif torch.is_tensor(boxes):
+        if boxes.dim() != 2:
+            raise ValueError(f"loss: ground-truth boxes of shape {tuple(boxes.shape)}; need (n, 9)")
+        out = torch.cat((boxes[:, :2], boxes[:, 2:3] + boxes[:, 5:6] * 0.5, boxes[:, 3:]), dim=1)
+    else:
+        raise TypeError(f"loss: ground-truth boxes of type {type(boxes).__name__}; need LiDARInstance3DBoxes-like "
+                        "objects or (n, 9) tensors")
+    if out.shape[1] != 9:
+        raise ValueError(f"loss: ground-truth boxes with {out.shape[1]} columns; need 9 (x, y, z, w, l, h, yaw, vx, "
+                         "vy)")
+    return out.float()
+
+
+def _to_device(host, device):
+    """A small host tensor on ``device`` without a synchronisation (pinned, non-blocking)."""
+    if device.type != "cuda":
+        return host
+    return host.pin_memory().to(device, non_blocking=True)
+
+
+def avg_factors(counts, num_layers, device, sync_cls_avg_factor):
+    """(num_layers * groups, 2) float32 avg factors before max(., 1), in device memory: ``counts[g]`` is
+    num_total_pos of group g (the same for every layer).  Column 1 (regression) is ``reduce_mean`` of the counts; column
+    0 (classification) too with ``sync_cls_avg_factor``, else the local count.  Under torch.distributed the mean is ONE
+    all_reduce of every slot's count divided by the world size, and nothing is read back."""
+    import torch.distributed as dist
+    host = torch.tensor(counts, dtype=torch.float32).repeat(num_layers)[:, None].repeat(1, 2)
+    avg = _to_device(host, device)
+    if dist.is_available() and dist.is_initialized():
+        red = avg[:, 1].clone().div_(dist.get_world_size())
+        dist.all_reduce(red)
+        avg[:, 1] = red
+        if sync_cls_avg_factor:
+            avg[:, 0] = red
+    return avg
+
+
+def _linear_sum_assignment():
+    try:
+        from scipy.optimize import linear_sum_assignment
+    except ImportError as e:
+        raise ImportError('Please run "pip install scipy" to install scipy first.') from e
+    return linear_sum_assignment
 
 
 class BEVFormerHead(nn.Module):
@@ -243,6 +351,73 @@ class BEVFormerHead(nn.Module):
             outputs_coords.append(tmp)
         return torch.stack(outputs_classes), torch.stack(outputs_coords)
 
+    def loss(self, gt_bboxes_list, gt_labels_list, preds_dicts, gt_bboxes_ignore=None, img_metas=None):
+        """bevformer_head.py:395-480: dict(loss_cls, loss_bbox, d0.loss_cls, d0.loss_bbox, ..., d{L-2}.*) of the
+        last and the earlier decoder layers.  ``gt_bboxes_list``: per sample, LiDARInstance3DBoxes-like objects or
+        (n, 9) tensors (``gravity_center_boxes``); ``gt_labels_list``: per sample, (n,) class indices.  Synchronises
+        with the host once (the cost matrix for scipy's assignment); not capturable."""
+        return self._loss(gt_bboxes_list, gt_labels_list, preds_dicts, gt_bboxes_ignore, 1)
+
+    def _loss(self, gt_bboxes_list, gt_labels_list, preds_dicts, gt_bboxes_ignore, groups):
+        assert gt_bboxes_ignore is None, \
+            f"{self.__class__.__name__} only supports for gt_bboxes_ignore setting to None."
+        if preds_dicts.get("enc_cls_scores") is not None or preds_dicts.get("enc_bbox_preds") is not None:
+            raise NotImplementedError("loss: encoder proposals (as_two_stage) have no implementation")
+        st = _loss_settings(self)
+        cls, box = preds_dicts["all_cls_scores"], preds_dicts["all_bbox_preds"]
+        L, bs, nq, ncls = cls.shape
+        if len(gt_bboxes_list) != bs or len(gt_labels_list) != bs:
+            raise ValueError(f"loss: {len(gt_bboxes_list)} box lists and {len(gt_labels_list)} label lists for a "
+                             f"batch of {bs}")
+        if nq % groups:
+            raise ValueError(f"loss: {nq} queries do not split into {groups} groups")
+        nqg = nq // groups
+        device = cls.device
+        # 1. the ground truth, padded to the batch's largest count
+        boxes = [gravity_center_boxes(b) for b in gt_bboxes_list]
+        n = [int(b.shape[0]) for b in boxes]
+        for b, lab in zip(boxes, gt_labels_list):
+            if lab.numel() != b.shape[0]:
+                raise ValueError(f"loss: {lab.numel()} labels for {b.shape[0]} boxes")
+        G = max(n)
+        gt = torch.zeros((bs, G, 9), dtype=torch.float32, device=device)
+        labels = torch.zeros((bs, G), dtype=torch.int64, device=device)
+        for i, (b, lab) in enumerate(zip(boxes, gt_labels_list)):
+            if n[i]:
+                gt[i, :n[i]].copy_(b, non_blocking=True)
+                labels[i, :n[i]].copy_(lab.reshape(-1), non_blocking=True)
+        n_gt = _to_device(torch.tensor(n, dtype=torch.int32), device)
+        # num_total_pos of each group is known from the shapes: every sample matches min(n_gt, queries per group)
+        avg = avg_factors([sum(min(k, nqg) for k in n)] * groups, L, device, self.sync_cls_avg_factor)
+        # 2-4. one cost launch, one device-to-host copy, scipy per (layer, group, sample)
+        assign = torch.full((L * bs, nq), -1, dtype=torch.int32)
+        if G:
+            cost = ops.det_match_cost(cls, box, gt, labels, n_gt, st["cost_reg_kind"], st["cls_cost_weight"],
+                                      st["reg_cost_weight"], st["cost_alpha"], st["cost_gamma"],
+                                      st["cost_eps"]).cpu().numpy()
+            lsa = _linear_sum_assignment()
+            a = assign.numpy()
+            for p in range(L * bs):
+                k = n[p % bs]
+                if not k:
+                    continue
+                for g in range(groups):
+                    rows, cols = lsa(cost[p, g * nqg:(g + 1) * nqg, :k])
+                    a[p, g * nqg + rows] = cols
+        # 5-6. the assignment back to the device, one loss launch
+        assign = _to_device(assign, device)
+        cfg = dict(groups=groups, reg_kind=st["reg_kind"], cls_loss_weight=st["cls_loss_weight"],
+                   bbox_loss_weight=st["bbox_loss_weight"], alpha=st["alpha"], gamma=st["gamma"], beta=st["beta"])
+        slots = ops.DetLoss.apply(cls, box, assign, gt, labels, n_gt, self.code_weights.float(), avg, cfg)
+        # GroupDETR: each layer's losses summed over groups divided by group_detr (bevformer_head.py:666-682)
+        per_layer = slots if groups == 1 else (slots.view(L, groups, 2) / groups).sum(1)
+        layers = [row.unbind(0) for row in per_layer.unbind(0)]
+        loss_dict = {"loss_cls": layers[-1][0], "loss_bbox": layers[-1][1]}
+        for i, (lc, lb) in enumerate(layers[:-1]):
+            loss_dict[f"d{i}.loss_cls"] = lc
+            loss_dict[f"d{i}.loss_bbox"] = lb
+        return loss_dict
+
     def get_bboxes(self, preds_dicts, img_metas, rescale=False):
         """bevformer_head.py:482-509: [[bboxes, scores, labels]] per sample, boxes with a bottom-centre z.  The
         boxes are wrapped in ``img_metas[i]['box_type_3d']`` when the meta carries one, else the (n, 9) tensor."""
@@ -269,6 +444,12 @@ class BEVFormerHead_GroupDETR(BEVFormerHead):
     def _object_query_embeds(self, dtype):
         q = self.query_embedding.weight.to(dtype)
         return q if self.training else q[:self.num_query // self.group_detr]
+
+    def loss(self, gt_bboxes_list, gt_labels_list, preds_dicts, gt_bboxes_ignore=None, img_metas=None):
+        """bevformer_head.py:603-683: ``BEVFormerHead.loss`` per group of ``num_query // group_detr`` queries, each
+        layer's losses summed over the groups divided by ``group_detr``.  Still one cost launch, one synchronisation
+        and one loss launch for all groups."""
+        return self._loss(gt_bboxes_list, gt_labels_list, preds_dicts, gt_bboxes_ignore, self.group_detr)
 
 
 _register(POSITIONAL_ENCODING, LearnedPositionalEncoding)

@@ -734,6 +734,69 @@ BEVF_API int bevf_nms_free_decode(const void *cls, int cls_dtype, const void *bo
                                   float *scores, int64_t *labels, int *num, void *stream);
 BEVF_API int64_t bevf_nms_free_decode_smem_bytes(int nq, int ncls, int max_num);
 
+/*
+ * Training loss of BEVFormerHead / BEVFormerHead_GroupDETR around a host-side Hungarian assignment.
+ * Common arguments:
+ *   cls        (P, nq, ncls) logits, box (P, nq, 10) normalised boxes, contiguous, any dtype code (widened to fp32);
+ *              P = L * bs, row p = l * bs + b (all_cls_scores / all_bbox_preds flattened over layer and sample)
+ *   gt         (bs, G, 9) f32 gravity-centred boxes (x, y, z, w, l, h, rot, vx, vy), gt_labels (bs, G) int64,
+ *              n_gt (bs) int32: sample b's first n_gt[b] boxes are real, the rest padding; the kernels normalise
+ *              them (normalize_bbox, core/bbox/util.py:4-24: cx, cy, log w, log l, cz, log h, sin rot, cos rot, vx, vy)
+ *   reg_kind   BEVF_DET_REG_L1 (BBox3DL1Cost / L1Loss) or BEVF_DET_REG_SMOOTH_L1 (SmoothL1Cost / SmoothL1Loss)
+ *   alpha, gamma  the focal parameters (mmdet's FocalLossCost / FocalLoss)
+ * The sigmoid is rounded to fp32 as torch.sigmoid computes it (libdevice expf, IEEE division), as are 1 - p and
+ * p + eps; the rest is evaluated in double and rounded once.
+ */
+enum bevf_det_reg { BEVF_DET_REG_L1 = 0, BEVF_DET_REG_SMOOTH_L1 = 1 };
+
+/*
+ * HungarianAssigner3D.assign's cost (core/bbox/assigners/hungarian_assigner_3d.py:106-116) for every (layer, sample)
+ * in one launch:
+ *   cost[p, q, g] = cls_weight * (pos - neg)[label_g] + reg_weight * reg(box[p, q, :8], normalize_bbox(gt[b, g])[:8])
+ *   pos = -log(p + eps) alpha (1 - p)^gamma, neg = -log(1 - p + eps) (1 - alpha) p^gamma   (mmdet 2.14 FocalLossCost)
+ *   reg = sum |d| (BBox3DL1Cost, match_costs/match_cost.py:7-29) or sum smooth-L1(d, beta 1) (SmoothL1Cost, :32-90)
+ * cost (P, nq, G) f32; columns g >= n_gt[b] are 0 and a label outside [0, ncls) gives NaN.  Query groups are ranges
+ * of q.  1 <= ncls <= 64, G >= 1 and bevf_det_match_cost_smem_bytes(ncls, G) <= 200 KiB.
+ */
+BEVF_API int bevf_det_match_cost(const void *cls, int cls_dtype, const void *box, int box_dtype, const float *gt,
+                                 const int64_t *gt_labels, const int *n_gt, float *cost, int P, int bs, int nq,
+                                 int ncls, int G, int reg_kind, float cls_weight, float reg_weight, float alpha,
+                                 float gamma, float eps, void *stream);
+BEVF_API int64_t bevf_det_match_cost_smem_bytes(int ncls, int G);
+
+/*
+ * BEVFormerHead.loss_single after the assignment (dense_heads/bevformer_head.py:215-393) for every slot s = l * groups
+ * + group in one launch; the slot's rows are (b, q) for all samples and q in [group * nq / groups, (group + 1) * nq /
+ * groups).
+ *   assign     (P, nq) int32: the ground-truth index matched to the query, or -1 (PseudoSampler: matched rows are
+ *              positive, with label gt_labels[b, assign]; the others have label num_classes = ncls)
+ *   loss_cls   mmcv 1.4's CUDA sigmoid_focal_loss (-alpha (1-p)^gamma log(max(p, FLT_MIN)) on the label's channel,
+ *              -(1-alpha) p^gamma log(max(1-p, FLT_MIN)) on the others), summed, / max(avg[s, 0], 1) * cls_loss_weight
+ *   loss_bbox  sum over positive rows whose normalised target is all finite (the reference's isnotnan) of
+ *              code_weights[c] * l(box - target) with l = |d| or smooth-L1 (beta), / max(avg[s, 1], 1)
+ *              * bbox_loss_weight
+ *   code_weights (10) f32; avg (S, 2) f32 in device memory; loss (S, 2) = nan_to_num of the values, loss_raw (S, 2) the
+ *   values before it (the backward reads them).  S = L * groups; one CTA per slot, fixed-order double sums.
+ */
+BEVF_API int bevf_det_loss_forward(const void *cls, int cls_dtype, const void *box, int box_dtype, const int *assign,
+                                   const float *gt, const int64_t *gt_labels, const int *n_gt,
+                                   const float *code_weights, const float *avg, float *loss, float *loss_raw, int L,
+                                   int bs, int nq, int groups, int ncls, int G, int reg_kind, float cls_loss_weight,
+                                   float bbox_loss_weight, float alpha, float gamma, float beta, void *stream);
+
+/*
+ * Gradient of bevf_det_loss_forward's slot scalars: grad_loss (S, 2) f32 is the upstream gradient of loss; a slot
+ * whose loss_raw is not finite passes none (nan_to_num).  grad_cls (P, nq, ncls) in cls_dtype (mmcv's analytic
+ * focal backward), grad_box (P, nq, 10) in box_dtype (sign(d), or d / beta inside smooth-L1's quadratic zone, times
+ * code_weights; zero on rows the forward dropped).  Every element is written once: no atomics.
+ */
+BEVF_API int bevf_det_loss_backward(const void *cls, int cls_dtype, const void *box, int box_dtype, const int *assign,
+                                    const float *gt, const int64_t *gt_labels, const int *n_gt,
+                                    const float *code_weights, const float *avg, const float *loss_raw,
+                                    const float *grad_loss, void *grad_cls, void *grad_box, int L, int bs, int nq,
+                                    int groups, int ncls, int G, int reg_kind, float cls_loss_weight,
+                                    float bbox_loss_weight, float alpha, float gamma, float beta, void *stream);
+
 #ifdef __cplusplus
 }
 #endif
