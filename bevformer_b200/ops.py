@@ -1106,18 +1106,27 @@ def point_sampling(lidar2img, pc_range, z_norm, img_h, img_w, bev_h, bev_w, raw_
 def linear_tc(x, weight, bias=None, residual=None, relu=False, out_dtype=None):
     """y = act(x @ weight.T + bias) (+ residual) on the wgmma GEMM.  x (..., K) and weight (N, K) both bf16 or
     both fp16, bias (N) any float dtype, residual (..., N) in x's dtype; returns (..., N) in x's dtype (default)
-    or fp32."""
+    or fp32.  Strided operands are copied to contiguous ones first."""
+    x = x.contiguous()
     _need_cuda(x, "x")
     if x.dtype not in TC_DTYPES or weight.dtype != x.dtype:
         raise RuntimeError("linear_tc: x and weight must be both bfloat16 or both float16")
     K = x.shape[-1]
+    if weight.dim() != 2 or weight.shape[1] != K:
+        raise RuntimeError(f"linear_tc: weight must be (N, {K}) for x (..., {K}), got {tuple(weight.shape)}")
     N = weight.shape[0]
     M = x.numel() // K
+    out_shape = x.shape[:-1] + (N,)
+    if bias is not None and (bias.dim() != 1 or bias.shape[0] != N):
+        raise RuntimeError(f"linear_tc: bias must be ({N},), got {tuple(bias.shape)}")
+    if residual is not None and (residual.dtype != x.dtype or residual.shape != out_shape):
+        raise RuntimeError(f"linear_tc: residual must be {tuple(out_shape)} in {x.dtype}, got "
+                           f"{tuple(residual.shape)} in {residual.dtype}")
     w = weight.contiguous()
     bq, bdt = (None, F32) if bias is None else _param_ptr(bias, x.dtype)
     res = None if residual is None else residual.contiguous()
     out_dtype = out_dtype or x.dtype
-    y = torch.empty(x.shape[:-1] + (N,), device=x.device, dtype=out_dtype)
+    y = torch.empty(out_shape, device=x.device, dtype=out_dtype)
     lib = _lib.load()
     with torch.cuda.device(x.device):
         st = lib.bevf_linear_forward_dt(x.data_ptr(), w.data_ptr(), _ptr(bq), bdt, _ptr(res), y.data_ptr(),
@@ -1155,16 +1164,23 @@ def linear_dgrad_tc(dy, weight, addend=None):
     return dx
 
 
+def _wgrad_operands(dy, x, who):
+    """dy (M, N) and x (M, K) as contiguous CUDA tensors of one tensor-core dtype: (dy, x, M, N, K)."""
+    if dy.dim() != 2 or x.dim() != 2:
+        raise RuntimeError(f"{who}: dy (M,N) and x (M,K) must be 2-D, got {tuple(dy.shape)} and {tuple(x.shape)}")
+    dy, x = dy.contiguous(), x.contiguous()
+    _need_cuda(dy, "dy")
+    _need_cuda(x, "x")
+    if dy.dtype not in TC_DTYPES or x.dtype != dy.dtype or dy.shape[0] != x.shape[0]:
+        raise RuntimeError(f"{who}: dy (M,N) and x (M,K) must be both bfloat16 or both float16 with equal M")
+    return dy, x, dy.shape[0], dy.shape[1], x.shape[1]
+
+
 def linear_wgrad_tc(dy, x, with_bias=False, out_dtype=None):
     """dW = dy^T @ x on the wgmma split-M kernel (and db = column sums of dy from the same pass).
     dy (M, N), x (M, K) both bf16 or both fp16 -> (N, K) fp32 [, (N,) fp32].  The kernel accumulates in one fp32
     buffer holding [dW | db]; ``out_dtype`` converts that buffer once (dW and db are views of it)."""
-    _need_cuda(dy, "dy")
-    _need_cuda(x, "x")
-    if dy.dtype not in TC_DTYPES or x.dtype != dy.dtype or dy.shape[0] != x.shape[0]:
-        raise RuntimeError("linear_wgrad_tc: dy (M,N) and x (M,K) must be both bfloat16 or both float16 with equal M")
-    M, N = dy.shape
-    K = x.shape[1]
+    dy, x, M, N, K = _wgrad_operands(dy, x, "linear_wgrad_tc")
     npad = (N + 3) // 4 * 4
     buf = torch.zeros(N * K + (npad if with_bias else 0), device=x.device, dtype=torch.float32)
     dw = buf[: N * K].view(N, K)
@@ -1180,14 +1196,11 @@ def linear_wgrad_tc(dy, x, with_bias=False, out_dtype=None):
 def linear_wgrad_into(dy, x, dw_acc, db_acc=None):
     """dW += dy^T @ x (and db += column sums of dy) accumulated into caller-provided fp32 buffers (the
     gradient arena): no allocation, no zero-fill, no conversion here."""
-    _need_cuda(dy, "dy")
-    _need_cuda(x, "x")
-    if dy.dtype not in TC_DTYPES or x.dtype != dy.dtype or dy.shape[0] != x.shape[0]:
-        raise RuntimeError("linear_wgrad_into: dy (M,N) and x (M,K) must be both bfloat16 or both float16 with equal M")
-    M, N = dy.shape
-    K = x.shape[1]
+    dy, x, M, N, K = _wgrad_operands(dy, x, "linear_wgrad_into")
     if dw_acc.dtype != torch.float32 or dw_acc.numel() != N * K or not dw_acc.is_contiguous():
         raise RuntimeError("linear_wgrad_into: dw_acc must be a contiguous fp32 (N, K) buffer")
+    if db_acc is not None and (db_acc.dtype != torch.float32 or db_acc.numel() != N or not db_acc.is_contiguous()):
+        raise RuntimeError("linear_wgrad_into: db_acc must be a contiguous fp32 (N,) buffer")
     _wgrad_acc(dy, x, dw_acc, db_acc)
 
 
@@ -1211,12 +1224,10 @@ def _wgrad_acc(dy, x, dw, db):
 
 def linear_wgrad_out(dy, x, grad_dtype, with_bias):
     """Two-pass weight (+ bias) gradient written directly in ``grad_dtype``: returns (dW, db|None)."""
-    _need_cuda(dy, "dy")
-    _need_cuda(x, "x")
-    if dy.dtype not in TC_DTYPES or x.dtype != dy.dtype or dy.shape[0] != x.shape[0]:
-        raise RuntimeError("linear_wgrad_out: dy (M,N) and x (M,K) must be both bfloat16 or both float16 with equal M")
-    M, N = dy.shape
-    K = x.shape[1]
+    dy, x, M, N, K = _wgrad_operands(dy, x, "linear_wgrad_out")
+    if M == 0:
+        return (torch.zeros((N, K), device=x.device, dtype=grad_dtype),
+                torch.zeros((N,), device=x.device, dtype=grad_dtype) if with_bias else None)
     lib = _lib.load()
     with torch.cuda.device(x.device):
         need = int(lib.bevf_linear_wgrad_workspace_bytes(M, N, K))
