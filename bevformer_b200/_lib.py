@@ -139,6 +139,10 @@ SIGNATURES = {
                               + [ctypes.c_float] * 5 + [c_void_p]),
     "bevf_det_loss_backward": (c_int, [c_void_p, c_int, c_void_p, c_int] + [c_void_p] * 10 + [c_int] * 7
                                + [ctypes.c_float] * 5 + [c_void_p]),
+    "bevf_dcn_sampling_forward": (c_int, [c_void_p] * 3 + [c_int, c_void_p] + [c_int] * 15 + [c_void_p]),
+    "bevf_dcn_sampling_backward": (c_int, [c_void_p] * 4 + [c_int] + [c_void_p] * 3 + [c_int] * 15 + [c_void_p]),
+    "bevf_dcn_sampling_backward_fx": (c_int, [c_void_p] * 4 + [c_int, c_void_p, c_void_p, c_int, c_void_p, c_void_p]
+                                      + [c_int] * 15 + [c_void_p]),
 }
 
 
@@ -176,7 +180,7 @@ def load(build_if_missing: bool = True):
     return _lib
 
 
-ABI_VERSION = 3
+ABI_VERSION = 4
 
 
 def check(status: int, lib=None) -> None:

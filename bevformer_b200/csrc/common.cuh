@@ -210,6 +210,12 @@ __host__ __device__ __forceinline__ int fx_exponent(unsigned a_bits, unsigned g_
     const int eg = (int)(g_bits >> 23 > 1u ? g_bits >> 23 : 1u) - 126;
     return ea + eg;
 }
+// |x| as sign-cleared float bits, the form the bounds words hold
+__device__ __forceinline__ unsigned abs_bits(float x) { return __float_as_uint(x) & 0x7fffffffu; }
+__device__ __forceinline__ unsigned abs_bits(bf16 x) {
+    return ((unsigned)__bfloat16_as_ushort(x) << 16) & 0x7fffffffu;
+}
+__device__ __forceinline__ unsigned abs_bits(__half x) { return abs_bits(__half2float(x)); }
 // 2^e as a double, -1022 <= e <= 1023
 __device__ __forceinline__ double fx_pow2(int e) { return __longlong_as_double((long long)(1023 + e) << 52); }
 // one contribution q * g (exact in double: two fp32 factors) scaled by a power of two and rounded to nearest

@@ -12,12 +12,6 @@ namespace bevf {
 
 constexpr int kFxThreads = 256;
 
-__device__ __forceinline__ unsigned abs_bits(float x) { return __float_as_uint(x) & 0x7fffffffu; }
-__device__ __forceinline__ unsigned abs_bits(bf16 x) {
-    return ((unsigned)__bfloat16_as_ushort(x) << 16) & 0x7fffffffu;
-}
-__device__ __forceinline__ unsigned abs_bits(__half x) { return abs_bits(__half2float(x)); }
-
 // one warp per query row; rows with row_map < 0 (unused rows of a fixed-capacity list, never written) are skipped
 template <typename TG>
 __global__ void __launch_bounds__(kFxThreads)

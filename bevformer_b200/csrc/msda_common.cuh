@@ -19,12 +19,10 @@ struct Corner {
     bool valid;
 };
 
-// Range test in float BEFORE any int conversion: projected anchors behind a camera reach |x| ~ 1e9.
-__device__ __forceinline__ Corner make_corner(float locx, float locy, int H, int W) {
+// Corner of the sample at pixel coordinates (x, y) (pixel centres at integers).  Range test in float BEFORE any int
+// conversion: projected anchors behind a camera reach |x| ~ 1e9.
+__device__ __forceinline__ Corner corner_at(float x, float y, int H, int W) {
     Corner c;
-    // unfused multiply / add: the sampling cell is floor(x), so x must round exactly like the
-    // reference expression loc * W - 0.5 (an FMA would flip floor() for samples on a cell boundary)
-    float x = __fadd_rn(__fmul_rn(locx, (float)W), -0.5f), y = __fadd_rn(__fmul_rn(locy, (float)H), -0.5f);
     c.valid = (x > -1.f) && (y > -1.f) && (x < (float)W) && (y < (float)H);
     if (!c.valid) { x = 0.f; y = 0.f; }
     const float xf = floorf(x), yf = floorf(y);
@@ -47,6 +45,13 @@ __device__ __forceinline__ Corner make_corner(float locx, float locy, int H, int
     c.dx = (x0ok && x1ok) ? 1 : 0;
     c.dy = (y0ok && y1ok) ? 1 : 0;
     return c;
+}
+
+// Corner of the sample at normalised location (locx, locy) of an H x W map.
+__device__ __forceinline__ Corner make_corner(float locx, float locy, int H, int W) {
+    // unfused multiply / add: the sampling cell is floor(x), so x must round exactly like the
+    // reference expression loc * W - 0.5 (an FMA would flip floor() for samples on a cell boundary)
+    return corner_at(__fadd_rn(__fmul_rn(locx, (float)W), -0.5f), __fadd_rn(__fmul_rn(locy, (float)H), -0.5f), H, W);
 }
 
 __device__ __forceinline__ void load_levels(const int64_t *level_hw, const int64_t *level_start,

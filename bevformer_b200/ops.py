@@ -1817,3 +1817,174 @@ class DetLoss(Function):
                                             grad_box.data_ptr(), *tail)
         _lib.check(st, lib)
         return grad_cls, grad_box, None, None, None, None, None, None, None
+
+
+# ---- modulated deformable convolution (DCNv2) ---------------------------------------------------------------------
+def _dcn_geom(input, offset, mask, weight, stride, padding, dilation, groups, deform_groups):
+    """(N, H, W, C, Ho, Wo, kh, kw, sh, sw, ph, pw, dh, dw, dg) of a modulated_deform_conv2d call, after mmcv's
+    argument checks and the kernels' alignment constraints."""
+    def pair(v):
+        return (int(v), int(v)) if isinstance(v, int) else tuple(int(x) for x in v)
+    if groups != 1:
+        raise NotImplementedError("modulated_deform_conv2d: groups != 1 is not implemented")
+    if input.dim() != 4 or weight.dim() != 4 or offset.dim() != 4 or mask.dim() != 4:
+        raise RuntimeError("modulated_deform_conv2d: input, offset, mask and weight must be 4-D")
+    if input.dtype not in _DT:
+        raise RuntimeError("modulated_deform_conv2d: input must be float32, bfloat16 or float16")
+    N, C, H, W = input.shape
+    Cout, Cw, kh, kw = weight.shape
+    (sh, sw), (ph, pw), (dh, dw) = pair(stride), pair(padding), pair(dilation)
+    dg, kk = int(deform_groups), kh * kw
+    if Cw != C:
+        raise RuntimeError(f"modulated_deform_conv2d: weight has {Cw} input channels, input has {C}")
+    if min(sh, sw, dh, dw, dg) <= 0 or min(ph, pw) < 0:
+        raise RuntimeError("modulated_deform_conv2d: stride, dilation and deform_groups must be positive, padding >= 0")
+    if C % dg:
+        raise RuntimeError(f"modulated_deform_conv2d: in_channels {C} is not divisible by deform_groups {dg}")
+    Ho = (H + 2 * ph - dh * (kh - 1) - 1) // sh + 1
+    Wo = (W + 2 * pw - dw * (kw - 1) - 1) // sw + 1
+    Ho, Wo = max(Ho, 0), max(Wo, 0)
+    if offset.shape[1] != 2 * dg * kk or mask.shape[1] != dg * kk:
+        raise RuntimeError(f"modulated_deform_conv2d: offset must have {2 * dg * kk} channels and mask {dg * kk} "
+                           f"(deform_groups * 2 * kh * kw, deform_groups * kh * kw), got {offset.shape[1]} and "
+                           f"{mask.shape[1]}")
+    if (offset.shape[0], mask.shape[0]) != (N, N) or tuple(offset.shape[2:]) != (Ho, Wo) or \
+            tuple(mask.shape[2:]) != (Ho, Wo):
+        raise RuntimeError(f"modulated_deform_conv2d: offset and mask must be ({N}, *, {Ho}, {Wo}) for this "
+                           f"convolution, got {tuple(offset.shape)} and {tuple(mask.shape)}")
+    vec = 16 // input.element_size()
+    if (C // dg) % vec:
+        raise RuntimeError(f"modulated_deform_conv2d: in_channels / deform_groups = {C // dg} must be a multiple of "
+                           f"{vec} in {input.dtype} (16-byte vector loads)")
+    if input.dtype in TC_DTYPES and ((kk * C) % 64 or Cout % 64):
+        raise RuntimeError(f"modulated_deform_conv2d: 16-bit storage needs kh * kw * in_channels ({kk * C}) and "
+                           f"out_channels ({Cout}) to be multiples of 64 (the wgmma GEMM's K and N)")
+    for t, n in ((input, "input"), (offset, "offset"), (mask, "mask"), (weight, "weight")):
+        if not t.is_cuda:
+            raise RuntimeError(f"modulated_deform_conv2d: {n} must be a CUDA tensor (bevformer_b200 has no CPU path)")
+    return N, H, W, C, Ho, Wo, kh, kw, sh, sw, ph, pw, dh, dw, dg
+
+
+def _channels_last(x: torch.Tensor) -> torch.Tensor:
+    """(N, C, H, W) -> contiguous (N, H, W, C): a view of a channels_last tensor, one transpose otherwise."""
+    return x.permute(0, 2, 3, 1).contiguous()
+
+
+def dcn_sampling_forward(x_nhwc, offset, mask, geom):
+    """Deformable im2col (bevf_dcn_sampling_forward): x (N, H, W, C), offset / mask in mmcv's layout, all of x's dtype
+    -> cols (N*Ho*Wo, kh*kw*C), column tap*C + c."""
+    N, H, W, C, Ho, Wo, kh, kw = geom[:8]
+    cols = torch.empty((N * Ho * Wo, kh * kw * C), device=x_nhwc.device, dtype=x_nhwc.dtype)
+    if cols.numel() == 0:
+        return cols
+    lib = _lib.load()
+    with torch.cuda.device(x_nhwc.device):
+        st = lib.bevf_dcn_sampling_forward(x_nhwc.data_ptr(), offset.data_ptr(), mask.data_ptr(), _DT[x_nhwc.dtype],
+                                           cols.data_ptr(), *geom, _stream_ptr(x_nhwc))
+    _lib.check(st, lib)
+    return cols
+
+
+def dcn_sampling_backward(x_nhwc, offset, mask, dcols, geom):
+    """Backward of the deformable im2col: (grad_input (N, H, W, C), grad_offset, grad_mask), all in x's dtype.
+    grad_input is summed with fp32 vector reductions, or -- under torch.use_deterministic_algorithms(True) -- in 64-bit
+    fixed point (bevf_dcn_sampling_backward_fx), which repeats bit for bit."""
+    N, H, W, C, Ho, Wo, kh, kw = geom[:8]
+    dev, dt = x_nhwc.device, x_nhwc.dtype
+    goff = torch.empty(offset.shape, device=dev, dtype=dt)
+    gmask = torch.empty(mask.shape, device=dev, dtype=dt)
+    if N * Ho * Wo == 0:
+        return torch.zeros(x_nhwc.shape, device=dev, dtype=dt), goff, gmask
+    lib = _lib.load()
+    common = (x_nhwc.data_ptr(), offset.data_ptr(), mask.data_ptr(), dcols.data_ptr(), _DT[dt])
+    with torch.cuda.device(dev):
+        if deterministic():
+            k = int(lib.bevf_msda_fx_frac_bits(Ho * Wo, 1, kh * kw))
+            fx = torch.zeros(x_nhwc.shape, device=dev, dtype=torch.int64)
+            bounds = torch.empty(2, device=dev, dtype=torch.int32)
+            st = lib.bevf_dcn_sampling_backward_fx(*common, fx.data_ptr(), bounds.data_ptr(), k, goff.data_ptr(),
+                                                   gmask.data_ptr(), *geom, _stream_ptr(x_nhwc))
+            _lib.check(st, lib)
+            gin = FixedPointGradValue(fx, bounds, k, dt).materialize()
+        else:
+            acc = torch.zeros(x_nhwc.shape, device=dev, dtype=torch.float32)
+            st = lib.bevf_dcn_sampling_backward(*common, acc.data_ptr(), goff.data_ptr(), gmask.data_ptr(), *geom,
+                                                _stream_ptr(x_nhwc))
+            _lib.check(st, lib)
+            gin = acc if dt == torch.float32 else acc.to(dt)
+    return gin, goff, gmask
+
+
+class ModulatedDeformConv2dFunction(Function):
+    """mmcv's ModulatedDeformConv2dFunction (mmcv/ops/modulated_deform_conv.py) on the library: the sampling kernels of
+    csrc/dcn.cu around the library's GEMMs -- y = cols . Wp^T (+ bias), Wp = weight.permute(0, 2, 3, 1) as
+    (Cout, kh*kw*Cin), on the wgmma kernel for bf16 / fp16 storage and on torch for fp32 (the parity configuration).
+    The backward recomputes the columns instead of saving them.  Input, offset, mask and weight share one dtype
+    (``modulated_deform_conv2d`` casts); the output is a channels_last (N, Cout, Ho, Wo) view of the GEMM's rows."""
+
+    @staticmethod
+    def forward(ctx, input, offset, mask, weight, bias=None, stride=1, padding=0, dilation=1, groups=1,
+                deform_groups=1):
+        geom = _dcn_geom(input, offset, mask, weight, stride, padding, dilation, groups, deform_groups)
+        N, H, W, C, Ho, Wo, kh, kw = geom[:8]
+        Cout = weight.shape[0]
+        x = _channels_last(input)
+        offset, mask = offset.contiguous(), mask.contiguous()
+        wp = weight.permute(0, 2, 3, 1).reshape(Cout, kh * kw * C).contiguous()
+        ctx.geom, ctx.has_bias = geom, bias is not None
+        ctx.dtypes = (weight.dtype, None if bias is None else bias.dtype)
+        ctx.save_for_backward(x, offset, mask, wp)
+        if N * Ho * Wo == 0:
+            return torch.empty((N, Cout, Ho, Wo), device=input.device, dtype=input.dtype)
+        cols = dcn_sampling_forward(x, offset, mask, geom)
+        if input.dtype in TC_DTYPES:
+            y = linear_tc(cols, wp, bias)
+        else:
+            y = cols @ wp.t()
+            if bias is not None:
+                y += bias
+        return y.view(N, Ho, Wo, Cout).permute(0, 3, 1, 2)
+
+    @staticmethod
+    @once_differentiable
+    def backward(ctx, grad_output):
+        x, offset, mask, wp = ctx.saved_tensors
+        geom = ctx.geom
+        N, H, W, C, Ho, Wo, kh, kw = geom[:8]
+        Cout = wp.shape[0]
+        dt = x.dtype
+        if N * Ho * Wo == 0:
+            return (torch.zeros((N, C, H, W), device=x.device, dtype=dt), torch.zeros_like(offset),
+                    torch.zeros_like(mask), torch.zeros((Cout, C, kh, kw), device=x.device, dtype=ctx.dtypes[0]),
+                    None if not ctx.has_bias else torch.zeros(Cout, device=x.device, dtype=ctx.dtypes[1]),
+                    None, None, None, None, None)
+        dy = grad_output.permute(0, 2, 3, 1).reshape(N * Ho * Wo, Cout).to(dt).contiguous()
+        cols = dcn_sampling_forward(x, offset, mask, geom)
+        if dt in TC_DTYPES:
+            dcols = linear_dgrad_tc(dy, wp)
+            if ctx.has_bias:
+                dwp, db = linear_wgrad_tc(dy, cols, with_bias=True)
+            else:
+                dwp, db = linear_wgrad_tc(dy, cols), None
+        else:
+            dcols = dy @ wp
+            dwp = dy.t() @ cols
+            db = colsum(dy) if ctx.has_bias else None
+        gin, goff, gmask = dcn_sampling_backward(x, offset, mask, dcols, geom)
+        grad_input = gin.permute(0, 3, 1, 2)
+        grad_weight = dwp.view(Cout, kh, kw, C).permute(0, 3, 1, 2).to(ctx.dtypes[0]).contiguous()
+        grad_bias = None if db is None else db.to(ctx.dtypes[1])
+        return grad_input, goff, gmask, grad_weight, grad_bias, None, None, None, None, None
+
+
+def modulated_deform_conv2d(input, offset, mask, weight, bias=None, stride=1, padding=0, dilation=1, groups=1,
+                            deform_groups=1):
+    """mmcv.ops.modulated_deform_conv2d with mmcv's argument order: out[n, co, ho, wo] = bias[co] +
+    sum_{c, i, j} weight[co, c, i, j] * mask[n, g*kk + i*kw + j, ho, wo] * bilinear(input[n, c], h, w)
+    (SURVEY.md Appendix B).  Computes in input's dtype: offset, mask and weight are cast to it (autograd returns
+    their gradients in their own dtypes); the bias may be any float dtype.  Returns (N, Cout, Ho, Wo) in
+    channels_last memory format."""
+    if input.is_floating_point() and input.dtype in _DT:
+        offset, mask, weight = (t.to(input.dtype) for t in (offset, mask, weight))
+    return ModulatedDeformConv2dFunction.apply(input, offset, mask, weight, bias, stride, padding, dilation, groups,
+                                               deform_groups)

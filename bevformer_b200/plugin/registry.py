@@ -90,6 +90,9 @@ def _registry(import_name, attr, name):
 HEADS = _registry("mmdet.models.builder", "HEADS", "head")
 BBOX_CODERS = _registry("mmdet.core.bbox.builder", "BBOX_CODERS", "bbox_coder")
 POSITIONAL_ENCODING = _registry("mmcv.cnn.bricks.registry", "POSITIONAL_ENCODING", "position encoding")
+# ModulatedDeformConv2dPack registers as 'DCNv2' where mmcv's own class does (mmcv/ops/modulated_deform_conv.py), and
+# replaces it there: mmdet's ResNet builds its dcn convs through mmcv.cnn's build_conv_layer
+CONV_LAYERS = _registry("mmcv.cnn.bricks.registry", "CONV_LAYERS", "conv layer")
 
 
 def _register(registry, cls, name=None):
@@ -102,6 +105,30 @@ def _register(registry, cls, name=None):
         except Exception:  # noqa: BLE001
             pass
     return cls
+
+
+if not HAVE_MMCV:     # what mmcv.cnn.bricks.conv registers
+    import torch.nn as _nn
+    for _name, _cls in (("Conv1d", _nn.Conv1d), ("Conv2d", _nn.Conv2d), ("Conv3d", _nn.Conv3d), ("Conv", _nn.Conv2d)):
+        CONV_LAYERS.register_module(name=_name, module=_cls)
+
+
+def build_conv_layer(cfg, *args, **kwargs):
+    """mmcv.cnn.build_conv_layer: the CONV_LAYERS class named by cfg['type'] (cfg None: nn.Conv2d), built with
+    ``*args, **kwargs`` plus the rest of cfg."""
+    if cfg is None:
+        cfg_ = dict(type="Conv2d")
+    else:
+        if not isinstance(cfg, dict):
+            raise TypeError("cfg must be a dict")
+        if "type" not in cfg:
+            raise KeyError('the cfg dict must contain the key "type"')
+        cfg_ = dict(cfg)
+    layer_type = cfg_.pop("type")
+    conv_layer = CONV_LAYERS.get(layer_type)
+    if conv_layer is None:
+        raise KeyError(f"Unrecognized conv type {layer_type}")
+    return conv_layer(*args, **kwargs, **cfg_)
 
 
 def build_attention(cfg, default_args=None):

@@ -40,7 +40,7 @@
 extern "C" {
 #endif
 
-#define BEVF_ABI_VERSION 3
+#define BEVF_ABI_VERSION 4
 
 #if defined(__GNUC__)
 #define BEVF_API __attribute__((visibility("default")))
@@ -796,6 +796,56 @@ BEVF_API int bevf_det_loss_backward(const void *cls, int cls_dtype, const void *
                                     const float *grad_loss, void *grad_cls, void *grad_box, int L, int bs, int nq,
                                     int groups, int ncls, int G, int reg_kind, float cls_loss_weight,
                                     float bbox_loss_weight, float alpha, float gamma, float beta, void *stream);
+
+/* ------------------------------------------------------------------------------------------------
+ * Modulated deformable convolution (DCNv2): the sampling half of modulated_deform_conv2d.  The GEMMs around it
+ * (y = cols . Wp^T + bias, dcols = dy . Wp, dWp = dy^T . cols) run on bevf_linear_forward_dt / _dgrad_dt / _wgrad_dt.
+ *
+ * replaces: the deformable im2col / col2im of mmcv._ext.modulated_deform_conv_forward / _backward (mmcv-full 1.4.0,
+ *   called from mmcv/ops/modulated_deform_conv.py), which ModulatedDeformConv2dPack ('DCNv2') runs in ResNet-101-DCN
+ *   (projects/configs/bevformer/bevformer_base.py:43-53, bevformer_small.py:50-61).  Semantics: SURVEY.md Appendix B.
+ *
+ * Common arguments (all tensors contiguous, one storage type `dtype` for every non-accumulator tensor):
+ *   input       (N, H, W, C)           channels-last, 16-byte aligned
+ *   offset      (N, dg * 2 * kk, Ho, Wo)  mmcv's layout: (y, x) pairs per tap, per deform group; kk = kh * kw
+ *   mask        (N, dg * kk, Ho, Wo)
+ *   cols/dcols  (N * Ho * Wo, kk * C)   column tap * C + c, tap = i * kw + j; 16-byte aligned
+ *   (Ho, Wo) must be the convolution's output size for (kh, kw, stride, padding, dilation); C % dg == 0 and the
+ *   channels of a deform group, C / dg, a multiple of 16 bytes (4 fp32 / 8 bf16 or fp16 values).  N * H * W,
+ *   H * W * C and Ho * Wo * kk below 2^31.  N * Ho * Wo == 0: nothing is launched.
+ * Sampling positions are one fp32 add of the exact integer base (ho * stride - pad + i * dil) and the widened offset;
+ * bilinear weights and zero padding as the sampler's (Appendix A); fp32 accumulation, one rounding to `dtype`.
+ */
+/* cols = mask * bilinear(input): fully overwritten (zeros for samples outside the map). */
+BEVF_API int bevf_dcn_sampling_forward(const void *input, const void *offset, const void *mask, int dtype, void *cols,
+                                       int N, int H, int W, int C, int Ho, int Wo, int kh, int kw, int sh, int sw,
+                                       int ph, int pw, int dh, int dw, int dg, void *stream);
+
+/*
+ * Backward of the sampling, given dcols (the input gradient of the column matrix):
+ *   grad_input   (N, H, W, C) f32 -- ACCUMULATED INTO (caller zero-fills) with 16-byte fp32 vector reductions; the
+ *                summation order is not deterministic (bevf_dcn_sampling_backward_fx below is the deterministic form)
+ *   grad_offset  (N, dg * 2 * kk, Ho, Wo) dtype, grad_mask (N, dg * kk, Ho, Wo) dtype -- fully overwritten; zero for
+ *                samples outside the map; each is one fixed-order fp32 sum over the group's channels
+ */
+BEVF_API int bevf_dcn_sampling_backward(const void *input, const void *offset, const void *mask, const void *dcols,
+                                        int dtype, float *grad_input, void *grad_offset, void *grad_mask, int N, int H,
+                                        int W, int C, int Ho, int Wo, int kh, int kw, int sh, int sw, int ph, int pw,
+                                        int dh, int dw, int dg, void *stream);
+
+/*
+ * Deterministic form: grad_input summed in 64-bit fixed point (int64, ACCUMULATED INTO, caller zero-fills), with
+ * the scale rule of bevf_msda_backward_fx: bounds (2,) u32 device words receive max|mask| and max|dcols| (written
+ * here), every contribution w * mask * dcol is stored as round(contribution * 2^(frac_bits - E)), E = fx_exponent of
+ * the bounds.  0 <= frac_bits <= bevf_msda_fx_frac_bits(Ho * Wo, 1, kk) (every sample of an image on one pixel).
+ * bevf_msda_fx_convert turns the sums into the input's dtype (NaN everywhere when a bound is not finite).
+ * grad_offset / grad_mask as above, bit for bit.
+ */
+BEVF_API int bevf_dcn_sampling_backward_fx(const void *input, const void *offset, const void *mask, const void *dcols,
+                                           int dtype, int64_t *grad_input_fx, uint32_t *bounds, int frac_bits,
+                                           void *grad_offset, void *grad_mask, int N, int H, int W, int C, int Ho,
+                                           int Wo, int kh, int kw, int sh, int sw, int ph, int pw, int dh, int dw,
+                                           int dg, void *stream);
 
 #ifdef __cplusplus
 }
