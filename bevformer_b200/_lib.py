@@ -1,11 +1,14 @@
-"""ctypes binding of ``libbevformer_b200.so`` (the C ABI declared in ``include/bevformer_b200.h``).
+"""ctypes binding of ``libbevformer_b200.so``, derived from the C ABI in ``include/bevformer_b200.h``.
 
-There is no fallback: if the library is missing and cannot be built, importing an op raises.
+The header is the one statement of the ABI: every ``BEVF_API`` prototype is bound with the ctypes types of its C
+types, and ``ABI_VERSION`` and the enum codes (``ENUMS``) are read from it.  There is no fallback: if the library is
+missing and cannot be built, importing an op raises.
 """
 from __future__ import annotations
 
 import ctypes
 import os
+import re
 import threading
 
 from . import build as _build
@@ -13,137 +16,42 @@ from . import build as _build
 _lock = threading.Lock()
 _lib = None
 
-c_void_p, c_int, c_int64 = ctypes.c_void_p, ctypes.c_int, ctypes.c_int64
+# the scalar C types the header passes by value; every pointer is a c_void_p.  Any other type raises at import, so a
+# new entry point with a new scalar type cannot bind wrongly.
+_SCALARS = {"int": ctypes.c_int, "int64_t": ctypes.c_int64, "uint64_t": ctypes.c_uint64, "float": ctypes.c_float,
+            "double": ctypes.c_double}
 
-# name -> (restype, argtypes); mirrors include/bevformer_b200.h one to one
-SIGNATURES = {
-    "bevf_version": (c_int, []),
-    "bevf_last_error": (ctypes.c_char_p, []),
-    "bevf_launch_count": (c_int64, []),
-    "bevf_msda_forward": (c_int, [c_void_p, c_int, c_void_p, c_void_p, c_void_p, c_void_p,
-                                  c_void_p, c_int] + [c_int] * 7 + [c_void_p]),
-    "bevf_msda_backward": (c_int, [c_void_p, c_int, c_void_p, c_void_p, c_void_p, c_void_p,
-                                   c_void_p, c_int, c_void_p, c_void_p, c_void_p] + [c_int] * 7
-                           + [c_void_p]),
-    "bevf_msda_rows_forward": (c_int, [c_void_p, c_int, c_void_p, c_void_p, c_void_p, c_void_p,
-                                       c_void_p, c_int, c_void_p] + [c_int] * 7 + [c_void_p]),
-    "bevf_msda_rows_backward": (c_int, [c_void_p, c_int, c_void_p, c_void_p, c_void_p, c_void_p,
-                                        c_void_p, c_int, c_void_p, c_void_p, c_void_p, c_void_p]
-                                + [c_int] * 7 + [c_void_p]),
-    "bevf_msda_rows_backward_ordered": (c_int, [c_void_p, c_int, c_void_p, c_void_p, c_void_p, c_void_p,
-                                                c_void_p, c_int, c_void_p, c_void_p, c_void_p, c_void_p,
-                                                c_void_p] + [c_int] * 7 + [c_void_p]),
-    "bevf_msda_set_backward_mode": (c_int, [c_int]),
-    "bevf_abs_max": (c_int, [c_void_p, c_int, c_int64, c_void_p, c_void_p]),
-    "bevf_msda_rows_backward_f16acc": (c_int, [c_void_p, c_int, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int,
-                                               c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p] + [c_int] * 7
-                                       + [c_void_p]),
-    "bevf_gv16_unscale": (c_int, [c_void_p, c_void_p, c_void_p, c_int64, c_void_p]),
-    "bevf_msda_rows_backward_mixed": (c_int, [c_void_p, c_int, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p,
-                                              c_int, c_void_p, c_void_p, c_void_p, c_int, c_void_p, c_void_p, c_void_p,
-                                              c_void_p] + [c_int] * 7 + [c_void_p]),
-    "bevf_msda_rows_backward_mixed_dense": (c_int, [c_void_p, c_int, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p,
-                                                    c_void_p, c_int, c_void_p, c_void_p, c_void_p, c_int, c_int,
-                                                    c_void_p, c_void_p, c_void_p, c_void_p] + [c_int] * 7 + [c_void_p]),
-    "bevf_gv_merge": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_void_p]),
-    "bevf_msda_fx_frac_bits": (c_int, [c_int64, c_int, c_int]),
-    "bevf_msda_backward_fx": (c_int, [c_void_p, c_int, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int,
-                                      c_void_p, c_void_p, c_int, c_void_p, c_void_p] + [c_int] * 7 + [c_void_p]),
-    "bevf_msda_rows_backward_fx": (c_int, [c_void_p, c_int, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int,
-                                           c_void_p, c_void_p, c_int, c_void_p, c_void_p, c_void_p] + [c_int] * 7
-                                   + [c_void_p]),
-    "bevf_msda_fx_convert": (c_int, [c_void_p, c_void_p, c_int, c_void_p, c_int, c_int, c_int64, c_void_p]),
-    "bevf_msda_rows_backward_dense": (c_int, [c_void_p, c_int, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p,
-                                              c_void_p, c_int, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p]
-                                      + [c_int] * 7 + [c_void_p]),
-    "bevf_msda_set_dense_backward": (c_int, [c_int]),
-    "bevf_msda_get_dense_backward": (c_int, []),
-    "bevf_msda_dense_plan": (c_int, [c_void_p, c_int, c_int, c_int, c_void_p, c_int, c_void_p]),
-    "bevf_sca_plan_workspace_ints": (c_int64, [c_int, c_int]),
-    "bevf_sca_plan_build": (c_int, [c_void_p] * 10 + [c_int] * 5 + [c_void_p]),
-    "bevf_sca_prep_forward": (c_int, [c_void_p] * 7 + [c_int] * 8 + [c_void_p]),
-    "bevf_sca_prep_backward": (c_int, [c_void_p] * 6 + [c_int] * 8 + [c_void_p]),
-    "bevf_sca_rows_forward_fused": (c_int, [c_void_p, c_int] + [c_void_p] * 9 + [c_int, c_void_p, c_int, c_void_p]
-                                    + [c_int] * 12 + [c_void_p]),
-    "bevf_sca_rows_backward_fused": (c_int, [c_void_p, c_int] + [c_void_p] * 7 + [c_int] + [c_void_p] * 5
-                                     + [c_int, c_void_p, c_void_p, c_void_p, c_int, c_int] + [c_void_p] * 5
-                                     + [c_int] * 12 + [c_void_p]),
-    "bevf_sca_prep_backward_multi": (c_int, [c_void_p] * 6 + [c_int] * 8 + [c_void_p]),
-    "bevf_tsa_prep_forward": (c_int, [c_void_p] * 5 + [c_int] * 6 + [c_void_p]),
-    "bevf_tsa_prep_backward": (c_int, [c_void_p] * 5 + [c_int] * 7 + [c_void_p]),
-    "bevf_query_prep_forward": (c_int, [c_void_p] * 5 + [c_int] * 7 + [c_void_p]),
-    "bevf_query_prep_backward": (c_int, [c_void_p] * 5 + [c_int] * 8 + [c_void_p]),
-    "bevf_refine_points": (c_int, [c_void_p, c_int64, c_void_p, c_void_p, c_void_p, c_int, c_int64, c_void_p]),
-    "bevf_layernorm_forward": (c_int, [c_void_p] * 4 + [c_int] + [c_void_p] * 5
-                               + [c_int64, c_int, ctypes.c_float, ctypes.c_float, ctypes.c_uint64, c_void_p,
-                                  c_int, c_void_p]),
-    "bevf_layernorm_backward": (c_int, [c_void_p] * 3 + [c_int] + [c_void_p] * 4 + [c_int64]
-                                + [c_void_p] * 4
-                                + [c_int64, c_int, ctypes.c_float, ctypes.c_uint64, c_void_p, c_int,
-                                   c_void_p]),
-    "bevf_layernorm_backward_workspace_bytes": (c_int64, [c_int64, c_int]),
-    "bevf_layernorm_backward_det": (c_int, [c_void_p] * 3 + [c_int] + [c_void_p] * 4 + [c_int64]
-                                    + [c_void_p] * 5 + [c_int64]
-                                    + [c_int64, c_int, ctypes.c_float, ctypes.c_uint64, c_void_p, c_int,
-                                       c_void_p]),
-    "bevf_sca_combine_forward": (c_int, [c_void_p] * 4 + [c_int] * 6 + [c_void_p]),
-    "bevf_sca_combine_backward": (c_int, [c_void_p] * 4 + [c_int] * 5 + [c_void_p]),
-    "bevf_linear_forward": (c_int, [c_void_p] * 3 + [c_int] + [c_void_p] * 2
-                            + [c_int, c_int64, c_int, c_int, c_int, c_void_p]),
-    "bevf_flatten_feats": (c_int, [c_void_p] * 4 + [c_int] * 7 + [c_void_p]),
-    "bevf_linear_dgrad": (c_int, [c_void_p] * 3 + [c_int64, c_int, c_int, c_void_p]),
-    "bevf_linear_dgrad_acc": (c_int, [c_void_p] * 4 + [c_int64, c_int, c_int, c_void_p]),
-    "bevf_linear_wgrad": (c_int, [c_void_p] * 4 + [c_int64, c_int, c_int, c_void_p]),
-    "bevf_linear_wgrad_workspace_bytes": (c_int64, [c_int64, c_int, c_int]),
-    "bevf_linear_wgrad_out": (c_int, [c_void_p] * 4 + [c_int, c_void_p, c_int64, c_int64, c_int, c_int,
-                                                      c_void_p]),
-    "bevf_sum_tensors": (c_int, [c_void_p, c_int, c_void_p, c_int64, c_int, c_void_p]),
-    "bevf_linear_wgrad_into": (c_int, [c_void_p] * 5 + [c_int64, c_int64, c_int, c_int, c_void_p]),
-    "bevf_linear_forward_dt": (c_int, [c_void_p] * 3 + [c_int] + [c_void_p] * 2
-                               + [c_int, c_int64, c_int, c_int, c_int, c_int, c_void_p]),
-    "bevf_linear_dgrad_dt": (c_int, [c_void_p] * 3 + [c_int64, c_int, c_int, c_int, c_void_p]),
-    "bevf_linear_dgrad_acc_dt": (c_int, [c_void_p] * 4 + [c_int64, c_int, c_int, c_int, c_void_p]),
-    "bevf_linear_wgrad_dt": (c_int, [c_void_p] * 4 + [c_int64, c_int, c_int, c_int, c_void_p]),
-    "bevf_linear_wgrad_out_dt": (c_int, [c_void_p] * 4 + [c_int, c_void_p, c_int64, c_int64, c_int, c_int, c_int,
-                                                         c_void_p]),
-    "bevf_linear_wgrad_into_dt": (c_int, [c_void_p] * 5 + [c_int64, c_int64, c_int, c_int, c_int, c_void_p]),
-    "bevf_colsum": (c_int, [c_void_p, c_void_p, c_int64, c_int, c_int, c_void_p]),
-    "bevf_colsum_workspace_bytes": (c_int64, [c_int64, c_int]),
-    "bevf_colsum_det": (c_int, [c_void_p, c_void_p, c_void_p, c_int64, c_int64, c_int, c_int, c_void_p]),
-    "bevf_dropout_inplace": (c_int, [c_void_p, c_int64, ctypes.c_float, ctypes.c_uint64, c_void_p, c_int,
-                                     c_void_p]),
-    "bevf_relu_dropout_backward": (c_int, [c_void_p, c_void_p, c_void_p, c_int64, ctypes.c_float, c_int,
-                                           c_void_p]),
-    "bevf_point_sampling": (c_int, [c_void_p, c_void_p, c_void_p, ctypes.c_float, ctypes.c_float,
-                                    c_void_p, c_void_p] + [c_int] * 5 + [c_void_p]),
-    "bevf_attn_forward": (c_int, [c_void_p, c_int64] * 4 + [c_void_p] + [c_int] * 6
-                          + [ctypes.c_float, ctypes.c_float, ctypes.c_uint64, c_void_p, c_int, c_void_p]),
-    "bevf_attn_backward": (c_int, [c_void_p, c_int64] * 5 + [c_void_p, c_void_p] + [c_void_p, c_int64] * 3
-                           + [c_int] * 6 + [ctypes.c_float, ctypes.c_float, ctypes.c_uint64, c_void_p, c_int,
-                                            c_void_p]),
-    "bevf_attn_dropout_mask": (c_int, [c_void_p] + [c_int] * 5 + [ctypes.c_float, ctypes.c_uint64, c_void_p,
-                                                                  c_void_p]),
-    "bevf_ego_motion": (c_int, [c_void_p, c_void_p, c_int, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int]
-                        + [ctypes.c_double] * 4 + [c_int, c_void_p]),
-    "bevf_rotate_bev": (c_int, [c_void_p, c_int, c_int64, c_int64, c_void_p, c_void_p] + [c_int] * 5 + [c_void_p]),
-    "bevf_det_branches_forward": (c_int, [c_void_p, c_int64, c_int64, c_int64, c_int, c_void_p, c_void_p, c_int,
-                                          c_void_p, c_int, c_void_p, c_void_p] + [c_int] * 6
-                                  + [ctypes.c_float, c_void_p, c_void_p]),
-    "bevf_nms_free_decode": (c_int, [c_void_p, c_int, c_void_p, c_int] + [c_int] * 5
-                             + [c_void_p, c_int, ctypes.c_double, c_int] + [c_void_p] * 5),
-    "bevf_nms_free_decode_smem_bytes": (c_int64, [c_int, c_int, c_int]),
-    "bevf_det_match_cost": (c_int, [c_void_p, c_int, c_void_p, c_int] + [c_void_p] * 4 + [c_int] * 6
-                            + [ctypes.c_float] * 5 + [c_void_p]),
-    "bevf_det_match_cost_smem_bytes": (c_int64, [c_int, c_int]),
-    "bevf_det_loss_forward": (c_int, [c_void_p, c_int, c_void_p, c_int] + [c_void_p] * 8 + [c_int] * 7
-                              + [ctypes.c_float] * 5 + [c_void_p]),
-    "bevf_det_loss_backward": (c_int, [c_void_p, c_int, c_void_p, c_int] + [c_void_p] * 10 + [c_int] * 7
-                               + [ctypes.c_float] * 5 + [c_void_p]),
-    "bevf_dcn_sampling_forward": (c_int, [c_void_p] * 3 + [c_int, c_void_p] + [c_int] * 15 + [c_void_p]),
-    "bevf_dcn_sampling_backward": (c_int, [c_void_p] * 4 + [c_int] + [c_void_p] * 3 + [c_int] * 15 + [c_void_p]),
-    "bevf_dcn_sampling_backward_fx": (c_int, [c_void_p] * 4 + [c_int, c_void_p, c_void_p, c_int, c_void_p, c_void_p]
-                                      + [c_int] * 15 + [c_void_p]),
-}
+
+def _ctype(decl: str, named: bool = True):
+    """ctypes type of a C parameter declaration (``named``: it ends in the parameter's name) or return type."""
+    if "*" in decl:
+        return ctypes.c_void_p
+    words = [w for w in decl.split() if w != "const"]
+    scalar = " ".join(words[:-1] if named else words)
+    if scalar not in _SCALARS:
+        raise RuntimeError(f"bevformer_b200: no ctypes type for the C type of {decl!r} in {_build.HEADER}")
+    return _SCALARS[scalar]
+
+
+def _parse_header(path: str):
+    with open(path) as f:
+        text = re.sub(r"/\*.*?\*/", "", f.read(), flags=re.S)
+    signatures = {}
+    for ret, name, args in re.findall(r"BEVF_API\s+([\w\s\*]+?)\b(bevf_\w+)\s*\(([^)]*)\)\s*;", text):
+        restype = ctypes.c_char_p if "".join(ret.split()) == "constchar*" else _ctype(ret, named=False)
+        params = [] if args.strip() == "void" else args.split(",")
+        signatures[name] = (restype, [_ctype(p) for p in params])
+    version = int(re.search(r"#define\s+BEVF_ABI_VERSION\s+(\d+)", text).group(1))
+    enums = {}
+    for body in re.findall(r"\benum\s+\w+\s*\{([^}]*)\}", text):
+        for item in filter(str.strip, body.split(",")):
+            key, value = item.split("=")              # every enumerator has an explicit integer value
+            enums[key.strip()] = int(value)
+    return signatures, version, enums
+
+
+# name -> (restype, argtypes) of every entry point; the ABI version; enumerator name -> code
+SIGNATURES, ABI_VERSION, ENUMS = _parse_header(_build.HEADER)
 
 
 def lib_path() -> str:
@@ -178,9 +86,6 @@ def load(build_if_missing: bool = True):
             raise RuntimeError(f"bevformer_b200: ABI mismatch (library {have}, binding {ABI_VERSION})")
         _lib = lib
     return _lib
-
-
-ABI_VERSION = 4
 
 
 def check(status: int, lib=None) -> None:

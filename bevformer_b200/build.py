@@ -16,6 +16,7 @@ CSRC = os.path.join(HERE, "csrc")
 LIB_DIR = os.path.join(HERE, "lib")
 LIB_PATH = os.path.join(LIB_DIR, "libbevformer_b200.so")
 STAMP = os.path.join(LIB_DIR, "build.stamp")
+HEADER = os.path.join(os.path.dirname(HERE), "include", "bevformer_b200.h")   # the C ABI; _lib binds from it
 
 NVCC_FLAGS = [
     "-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17",
@@ -34,7 +35,7 @@ def sources():
 def _digest() -> str:
     h = hashlib.sha256()
     files = sorted(os.path.join(CSRC, f) for f in os.listdir(CSRC))
-    files.append(os.path.join(os.path.dirname(HERE), "include", "bevformer_b200.h"))
+    files.append(HEADER)
     for f in files:
         with open(f, "rb") as fh:
             h.update(f.encode() + b"\0" + fh.read())

@@ -15,7 +15,7 @@ from torch.autograd.function import Function, once_differentiable
 
 from . import _lib
 
-F32, BF16, F16 = 0, 1, 2
+F32, BF16, F16 = _lib.ENUMS["BEVF_DTYPE_F32"], _lib.ENUMS["BEVF_DTYPE_BF16"], _lib.ENUMS["BEVF_DTYPE_F16"]
 _DT = {torch.float32: F32, torch.bfloat16: BF16, torch.float16: F16}
 # operand types of the tensor-core projections (fp32 accumulation for both)
 TC_DTYPES = (torch.bfloat16, torch.float16)
@@ -1311,7 +1311,8 @@ def relu_dropout_backward(dy, h, p):
 # Device-resident ego-motion (csrc/ego_motion.cu): the per-frame shift / rotation / CAN-bus block of
 # PerceptionTransformer.get_bev_features without host arithmetic.
 # ---------------------------------------------------------------------------------------------------
-EGO_DELTAS, EGO_CONTINUE, EGO_NEW_SCENE = 0, 1, 2
+EGO_DELTAS, EGO_CONTINUE, EGO_NEW_SCENE = (_lib.ENUMS["BEVF_EGO_DELTAS"], _lib.ENUMS["BEVF_EGO_CONTINUE"],
+                                          _lib.ENUMS["BEVF_EGO_NEW_SCENE"])
 
 
 def ego_state(device) -> torch.Tensor:
@@ -1694,7 +1695,7 @@ def nms_free_decode(cls_scores, bbox_preds, max_num, post_center_range, score_th
 # Detection loss (csrc/det_loss.cu): the matching cost of every (layer, sample) in one launch, and the focal /
 # L1 / smooth-L1 losses of every (layer, group) slot with their gradient.  The assignment between them is the host's.
 # ---------------------------------------------------------------------------------------------------
-DET_REG = {"l1": 0, "smooth_l1": 1}
+DET_REG = {"l1": _lib.ENUMS["BEVF_DET_REG_L1"], "smooth_l1": _lib.ENUMS["BEVF_DET_REG_SMOOTH_L1"]}
 
 
 def _det_preds(cls_scores, bbox_preds, who):

@@ -19,9 +19,12 @@
  *
  * Conventions
  *   - plain C: raw device pointers, sizes, an opaque cudaStream_t passed as void*; no torch types.
- *   - the caller owns every buffer; the library never allocates, frees or synchronises, and keeps no
- *     mutable global state besides a thread-local error string, so every call is re-entrant and
- *     safe under CUDA-graph capture.
+ *   - the caller owns every buffer; the library never allocates, frees or synchronises, and every call is
+ *     re-entrant and safe under CUDA-graph capture.  Its process-wide state is the launch counter
+ *     (bevf_launch_count), the sampler's backward and dense-backward modes (bevf_msda_set_backward_mode,
+ *     bevf_msda_set_dense_backward) with the second stream and events those modes fork onto, and one-time setup
+ *     (environment variables read at first use, the SM count, kernel shared-memory limits); the last error is
+ *     thread-local.
  *   - every function returns 0 on success, non-zero on error; bevf_last_error() then holds a
  *     message for the calling thread (the Python wrapper raises RuntimeError with it, which is
  *     what mmcv's TORCH_CHECK failures surface as).
@@ -30,6 +33,9 @@
  *     pointer that a kernel accesses with 16 B vectors, while scalar and atomic operands (LayerNorm's mean / rstd /
  *     dgamma / dbeta, bevf_colsum's out, inv_count) may sit at any float offset.
  *   - there is NO CPU implementation behind this ABI.
+ *   - the Python binding (bevformer_b200/_lib.py) is read from this file: the BEVF_API prototypes, BEVF_ABI_VERSION
+ *     and the enums.  Scalars are passed as int, int64_t, uint64_t, float or double, and every enumerator has an
+ *     explicit value.
  */
 #ifndef BEVFORMER_B200_H_
 #define BEVFORMER_B200_H_

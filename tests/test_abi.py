@@ -29,8 +29,48 @@ def test_library_builds_and_exports_every_declared_symbol():
         assert hasattr(lib, s), f"{s} declared in the header but not exported"
 
 
-def test_binding_covers_header_exactly():
+# type code of each ctypes type of the binding, and the C++ template that spells the same code for a C type
+_CODES = {ctypes.c_void_p: "p", ctypes.c_char_p: "s", ctypes.c_int: "i", ctypes.c_int64: "q", ctypes.c_uint64: "Q",
+          ctypes.c_float: "f", ctypes.c_double: "d"}
+_TYPE_CODES_CPP = r"""
+#include <cstdio>
+#include <string>
+#include "bevformer_b200.h"
+template <class T> struct code;                       // a type without a code does not compile
+template <class T> struct code<T *> { static constexpr char c = 'p'; };
+template <> struct code<int> { static constexpr char c = 'i'; };
+template <> struct code<int64_t> { static constexpr char c = 'q'; };
+template <> struct code<uint64_t> { static constexpr char c = 'Q'; };
+template <> struct code<float> { static constexpr char c = 'f'; };
+template <> struct code<double> { static constexpr char c = 'd'; };
+template <class T> struct ret : code<T> {};
+template <> struct ret<const char *> { static constexpr char c = 's'; };
+template <class F> struct sig;
+template <class R, class... A> struct sig<R (*)(A...)> {
+    static std::string str() { return std::string(1, ret<R>::c) + std::string{code<A>::c...}; }
+};
+int main() {
+"""
+
+
+def test_binding_covers_header_exactly(tmp_path):
+    """The binding has exactly the header's entry points, with the return and argument types the C++ compiler sees
+    in the header's prototypes."""
+    import shutil
+    import subprocess
     assert sorted(_lib.SIGNATURES) == sorted(declared_symbols())
+    cxx = shutil.which("c++") or shutil.which("g++")
+    if not cxx:
+        pytest.skip("no host C++ compiler on PATH")
+    src = tmp_path / "type_codes.cpp"
+    src.write_text(_TYPE_CODES_CPP + "".join(f'    std::printf("{n} %s\\n", sig<decltype(&{n})>::str().c_str());\n'
+                                             for n in _lib.SIGNATURES) + "}\n")
+    exe = tmp_path / "type_codes"
+    subprocess.run([cxx, "-std=c++17", "-I", os.path.join(ROOT, "include"), str(src), "-o", str(exe)], check=True)
+    compiled = dict(line.split() for line in subprocess.run([str(exe)], capture_output=True, text=True,
+                                                            check=True).stdout.splitlines())
+    bound = {n: _CODES[res] + "".join(_CODES[a] for a in args) for n, (res, args) in _lib.SIGNATURES.items()}
+    assert bound == compiled
 
 
 def test_version_and_error_channel():
