@@ -1989,3 +1989,44 @@ def modulated_deform_conv2d(input, offset, mask, weight, bias=None, stride=1, pa
         offset, mask, weight = (t.to(input.dtype) for t in (offset, mask, weight))
     return ModulatedDeformConv2dFunction.apply(input, offset, mask, weight, bias, stride, padding, dilation, groups,
                                                deform_groups)
+
+
+# ---- GridMask -----------------------------------------------------------------------------------------------------
+def grid_mask_apply(x, d, l, st_h, st_w, use_h, use_w, mode):
+    """x (planes, H, W) times GridMask's mask for the drawn integers (bevf_grid_mask): a new contiguous tensor in x's
+    dtype, bit for bit torch's ``x * mask.to(x.dtype)``.  No autograd."""
+    _need_cuda(x, "grid_mask input")
+    if x.dtype not in _DT:
+        raise RuntimeError(f"grid_mask: dtype {x.dtype} not supported (float32, bfloat16 or float16)")
+    if x.dim() != 3:
+        raise RuntimeError(f"grid_mask: expected (planes, H, W), got {tuple(x.shape)}")
+    planes, H, W = x.shape
+    out = torch.empty_like(x)
+    lib = _lib.load()
+    with torch.cuda.device(x.device):
+        st = lib.bevf_grid_mask(x.data_ptr(), out.data_ptr(), _DT[x.dtype], planes, H, W, int(d), int(l), int(st_h),
+                                int(st_w), int(bool(use_h)), int(bool(use_w)), int(mode), _stream_ptr(x))
+    _lib.check(st, lib)
+    return out
+
+
+class GridMaskFunction(Function):
+    """out = x * m for GridMask's mask m (grid_mask.py:90-122 with rotate = 1, offset = False); the backward is the
+    same kernel on grad_out.  Saves only the drawn integers."""
+
+    @staticmethod
+    def forward(ctx, x, d, l, st_h, st_w, use_h, use_w, mode):
+        ctx.args = (d, l, st_h, st_w, use_h, use_w, mode)
+        return grid_mask_apply(x.contiguous(), *ctx.args)
+
+    @staticmethod
+    @once_differentiable
+    def backward(ctx, grad_out):
+        return (grid_mask_apply(grad_out.contiguous(), *ctx.args),) + (None,) * 7
+
+
+def grid_mask(x, d, l, st_h, st_w, use_h=True, use_w=True, mode=0):
+    """GridMask's multiply for x (planes, H, W) in float32, bfloat16 or float16 on a CUDA device: row / column stripes
+    of period d and width l starting at st_h / st_w in the (1.5 H, 1.5 W) frame whose centre crop is the image, zeroed
+    (mode 0) or kept (mode 1).  Differentiable in x."""
+    return GridMaskFunction.apply(x, d, l, st_h, st_w, use_h, use_w, mode)

@@ -10,12 +10,13 @@ from .spatial_cross_attention import MSDeformableAttention3D, ScaPlan, SpatialCr
 from .temporal_self_attention import TemporalSelfAttention
 from .temporal import BEVStream, obtain_history_bev
 from .dcn import ModulatedDeformConv2d, ModulatedDeformConv2dPack
+from .grid_mask import GridMask
 from .head import BEVFormerHead, BEVFormerHead_GroupDETR, LearnedPositionalEncoding, NMSFreeCoder
 from .registry import BBOX_CODERS, CONV_LAYERS, HEADS, POSITIONAL_ENCODING, build_conv_layer
 from .transformer import (PerceptionTransformer, PerceptionTransformerBEVEncoder, PerceptionTransformerV2,
                           ResNetFusion)
 
-__all__ = ["ModulatedDeformConv2d", "ModulatedDeformConv2dPack", "CONV_LAYERS", "build_conv_layer", "BEVFormerHead", "BEVFormerHead_GroupDETR", "LearnedPositionalEncoding", "NMSFreeCoder", "HEADS",
+__all__ = ["GridMask", "ModulatedDeformConv2d", "ModulatedDeformConv2dPack", "CONV_LAYERS", "build_conv_layer", "BEVFormerHead", "BEVFormerHead_GroupDETR", "LearnedPositionalEncoding", "NMSFreeCoder", "HEADS",
            "BBOX_CODERS", "POSITIONAL_ENCODING", "PerceptionTransformerV2", "ResNetFusion", "BEVStream", "obtain_history_bev", "PerceptionTransformer", "PerceptionTransformerBEVEncoder", "CustomMSDeformableAttention", "DetectionTransformerDecoder",
            "DetrTransformerDecoderLayer", "GroupMultiheadAttention", "MultiheadAttention", "inverse_sigmoid", "BEVFormerEncoder", "BEVFormerLayer", "MyCustomBaseTransformerLayer", "FFN",
            "SpatialCrossAttention", "MSDeformableAttention3D", "TemporalSelfAttention", "ScaPlan",

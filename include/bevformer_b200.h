@@ -46,7 +46,7 @@
 extern "C" {
 #endif
 
-#define BEVF_ABI_VERSION 4
+#define BEVF_ABI_VERSION 5
 
 #if defined(__GNUC__)
 #define BEVF_API __attribute__((visibility("default")))
@@ -852,6 +852,26 @@ BEVF_API int bevf_dcn_sampling_backward_fx(const void *input, const void *offset
                                            void *grad_offset, void *grad_mask, int N, int H, int W, int C, int Ho,
                                            int Wo, int kh, int kw, int sh, int sw, int ph, int pw, int dh, int dw,
                                            int dg, void *stream);
+
+/* ------------------------------------------------------------------------------------------------
+ * GridMask, the detectors' training-time image mask (projects/mmdet3d_plugin/models/utils/grid_mask.py:70-124, built as
+ * GridMask(True, True, rotate=1, offset=False, ratio=0.5, mode=1, prob=0.7) by detectors/bevformer.py:52-53 and
+ * bevformerV2.py:54-55), applied without materialising the mask.
+ *
+ * replaces: the numpy stripe loop, the PIL round trip, the synchronising `.cuda()` copy of the mask and the multiply at
+ *   grid_mask.py:90-122 (rotate = 1, offset = False).
+ *
+ *   x, out   (planes, H, W) contiguous in `dtype` (f32 | bf16 | f16); out is fully overwritten and must not overlap x
+ *   d, l, st_h, st_w   the drawn stripe period, stripe width and start offsets: d >= 1, l >= 0, 0 <= st_h, st_w < d
+ * out[p, y, x] = x[p, y, x] * m[y, x], one mask for every plane.  With hh = int(1.5 * H), ww = int(1.5 * W),
+ * y' = y + (hh - H) / 2 and x' = x + (ww - W) / 2 (floor division), m is 0 when use_h != 0, k = (y' - st_h) / d lies
+ * in [0, hh / d) and (y' - st_h) % d < l (the row stripes the loop draws), or the same holds for x', st_w, ww and use_w;
+ * otherwise 1.  mode == 1 flips m.  The product is an fp32 multiply without flush-to-zero rounded once to `dtype`, as
+ * torch's x * mask.to(x.dtype) on the device: bit for bit equal to it, inf and NaN under a zero included.  The
+ * backward (grad_out * m) is the same call on grad_out.
+ */
+BEVF_API int bevf_grid_mask(const void *x, void *out, int dtype, int64_t planes, int H, int W, int d, int l, int st_h,
+                            int st_w, int use_h, int use_w, int mode, void *stream);
 
 #ifdef __cplusplus
 }
