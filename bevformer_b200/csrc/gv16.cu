@@ -6,6 +6,7 @@
 //   gv16_scale()        (common.cuh) the power of two that puts that maximum into [8, 16)
 //   bevf_gv16_unscale   fp16 accumulators -> bf16 gradient (divide by the scale), what the value projection consumes
 //   bevf_gv_merge       mixed mode: fine levels (scaled fp16) + coarse levels (fp32 side buffer) -> one bf16 gradient
+//   bevf_gv_merge_replicated   the same with replicated fp16 levels between them: their copies summed in fp32
 // Replaces nothing in the reference one to one: there grad_value is allocated in value's dtype and accumulated with
 // atomicAdd (multi_scale_deformable_attn_function.py:146-160); this is the same quantity, another accumulator format.
 #include <cuda_fp16.h>
@@ -64,27 +65,40 @@ gv16_unscale_kernel(const __half *__restrict__ gv16, const unsigned *__restrict_
     }
 }
 
-// out (B, S, row) bf16  <-  fine (B, S_fine, row) scaled fp16  |  side (B, S - S_fine, row) fp32; row = M * D elements
+// out (B, S, row) bf16  <-  f16 (B, S_fine + k * S_rep, row) scaled fp16  |  side (B, S - S_fine - S_rep, row) fp32;
+// row = M * D elements.  Pixel p < S_fine of a map is f16 pixel p; S_fine <= p < S_fine + S_rep is the sum of the k
+// copies p + c * S_rep of it (the replicated levels of msda_bwd_d32); the rest are side pixels from p - S_fine - S_rep.
 __global__ void __launch_bounds__(kGvThreads)
-gv_merge_kernel(const __half *__restrict__ fine, const float *__restrict__ side, const unsigned *__restrict__ amax,
-                bf16 *__restrict__ out, long long groups_per_map, long long fine_groups_per_map, long long total_groups) {
+gv_merge_kernel(const __half *__restrict__ f16, const float *__restrict__ side, const unsigned *__restrict__ amax,
+                bf16 *__restrict__ out, long long groups_per_map, long long fine_groups_per_map,
+                long long rep_groups_per_map, int k, long long total_groups) {
     // a group = 8 consecutive elements (16 B of bf16 output)
     const float inv = 1.f / gv16_scale(__ldg(amax));
-    const long long side_groups_per_map = groups_per_map - fine_groups_per_map;
+    const long long f16_groups_per_map = fine_groups_per_map + k * rep_groups_per_map;
+    const long long side_from = fine_groups_per_map + rep_groups_per_map;
+    const long long side_groups_per_map = groups_per_map - side_from;
     for (long long i = (long long)blockIdx.x * kGvThreads + threadIdx.x; i < total_groups; i += (long long)gridDim.x * kGvThreads) {
         const long long b = i / groups_per_map, r = i - b * groups_per_map;
         uint4 o;
-        if (r < fine_groups_per_map) {
-            const uint4 v = __ldg(reinterpret_cast<const uint4 *>(fine) + b * fine_groups_per_map + r);
-            const uint32_t w[4] = {v.x, v.y, v.z, v.w};
+        if (r < side_from) {
+            const uint4 *vp = reinterpret_cast<const uint4 *>(f16) + b * f16_groups_per_map + r;
+            float acc[8];
+            const int copies = r < fine_groups_per_map ? 1 : k;
+            for (int c = 0; c < copies; ++c) {
+                const uint4 v = __ldg(vp + c * rep_groups_per_map);
+                const uint32_t w[4] = {v.x, v.y, v.z, v.w};
+#pragma unroll
+                for (int j = 0; j < 4; ++j) {
+                    const float2 f = __half22float2(*reinterpret_cast<const __half2 *>(&w[j]));
+                    acc[2 * j] = c ? acc[2 * j] + f.x : f.x;
+                    acc[2 * j + 1] = c ? acc[2 * j + 1] + f.y : f.y;
+                }
+            }
             uint32_t *ow = &o.x;
 #pragma unroll
-            for (int j = 0; j < 4; ++j) {
-                const float2 f = __half22float2(*reinterpret_cast<const __half2 *>(&w[j]));
-                ow[j] = pack_bf16x2(f.x * inv, f.y * inv);
-            }
+            for (int j = 0; j < 4; ++j) ow[j] = pack_bf16x2(acc[2 * j] * inv, acc[2 * j + 1] * inv);
         } else {
-            const float4 *sp = reinterpret_cast<const float4 *>(side) + 2 * (b * side_groups_per_map + (r - fine_groups_per_map));
+            const float4 *sp = reinterpret_cast<const float4 *>(side) + 2 * (b * side_groups_per_map + (r - side_from));
             const float4 a = __ldg(sp), c = __ldg(sp + 1);
             o.x = pack_bf16x2(a.x, a.y); o.y = pack_bf16x2(a.z, a.w);
             o.z = pack_bf16x2(c.x, c.y); o.w = pack_bf16x2(c.z, c.w);
@@ -141,6 +155,27 @@ extern "C" int bevf_gv_merge(const void *fine_f16, const float *side_f32, const 
         return fail("%s: device pointers must be 16-byte aligned", who);
     const long long gpm = (long long)S * row_elems / 8, fpm = (long long)S_fine * row_elems / 8;
     gv_merge_kernel<<<gv_grid(gpm * B), kGvThreads, 0, (cudaStream_t)stream>>>((const __half *)fine_f16, side_f32, amax_bits,
-                                                                             (bf16 *)out_bf16, gpm, fpm, gpm * B);
+                                                                             (bf16 *)out_bf16, gpm, fpm, 0, 1, gpm * B);
+    return check_launch(who);
+}
+
+extern "C" int bevf_gv_merge_replicated(const void *f16, const float *side_f32, const uint32_t *amax_bits,
+                                        void *out_bf16, int B, int S, int S_fine, int S_rep, int replicas,
+                                        int row_elems, void *stream) {
+    const char *who = "bevf_gv_merge_replicated";
+    if (B < 0 || S <= 0 || S_fine <= 0 || S_rep < 0 || S_fine + S_rep > S || replicas < 1 || row_elems <= 0 ||
+        row_elems % 8)
+        return fail("%s: bad dimension (0 < S_fine, 0 <= S_rep, S_fine + S_rep <= S, replicas >= 1, row_elems a "
+                    "multiple of 8)", who);
+    if (B == 0) return 0;
+    const bool has_side = S_fine + S_rep < S;
+    if (!f16 || (has_side && !side_f32) || !amax_bits || !out_bf16) return fail("%s: null pointer argument", who);
+    if (!aligned16(f16) || !aligned16(side_f32) || !aligned16(out_bf16))
+        return fail("%s: device pointers must be 16-byte aligned", who);
+    const long long gpm = (long long)S * row_elems / 8, fpm = (long long)S_fine * row_elems / 8,
+                    rpm = (long long)S_rep * row_elems / 8;
+    gv_merge_kernel<<<gv_grid(gpm * B), kGvThreads, 0, (cudaStream_t)stream>>>((const __half *)f16, side_f32, amax_bits,
+                                                                             (bf16 *)out_bf16, gpm, fpm, rpm, replicas,
+                                                                             gpm * B);
     return check_launch(who);
 }

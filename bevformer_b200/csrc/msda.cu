@@ -175,7 +175,7 @@ msda_bwd_d32(const T *__restrict__ value, const int64_t *__restrict__ level_hw,
              const __grid_constant__ HostLevels host_levels, const unsigned *__restrict__ gv_amax = nullptr,
              __half *__restrict__ gv16 = nullptr, unsigned gv16_mask = 0u, int side_start = 0, int S_side = 0,
              const unsigned *__restrict__ fx_bounds = nullptr, int fx_bits = 0,
-             const __grid_constant__ ScaFuse fz = ScaFuse{}) {
+             const __grid_constant__ ScaFuse fz = ScaFuse{}, int rep_start = 0, int rep_k = 1) {
     // TV = long long: grad_value in 64-bit fixed point (deterministic mode): each lane adds VEC channels of every
     // corner contribution with scalar integer reductions, scaled by 2^(fx_bits - fx_exponent(fx_bounds)) (common.cuh);
     // non-finite bounds: nothing is scattered (the conversion then writes NaN)
@@ -184,6 +184,11 @@ msda_bwd_d32(const T *__restrict__ value, const int64_t *__restrict__ level_hw,
     // gv16 (B, side_start, M, 32); the other levels are the pixels [side_start, S) and accumulate in fp32 into
     // grad_value, which then is the SIDE buffer (B, S_side = S - side_start, M, 32).  side_start comes from the host's
     // copy of the pyramid; the level mask is re-derived from the device pyramid (below).
+    // Replicated fp16 levels (mixed mode, rep_start < side_start): the pixels [rep_start, side_start) -- levels with
+    // more contributions per pixel than one fp16 running sum holds accurately -- are accumulated in scaled fp16 too,
+    // into rep_k copies that follow the fine pixels in every map of gv16: (B, rep_start + rep_k * S_rep, M, 32),
+    // S_rep = side_start - rep_start; pair row r adds into copy r % rep_k, so each copy sums about 1 / rep_k of
+    // them (adjacent pair rows are adjacent queries, which hit the same coarse pixels).  The merge sums the copies.
     // red_skip: bit l set = the grad_value contributions of level l are NOT scattered here (hybrid mode: the
     // coarse levels go through msda_bwd_splat_d32, which merges them in registers, on a second stream)
     constexpr int VEC = Vec<T>::N, LANES = 32 / VEC, G = 32 / LANES;
@@ -197,22 +202,32 @@ msda_bwd_d32(const T *__restrict__ value, const int64_t *__restrict__ level_hw,
     __shared__ unsigned s_skip;
     if (threadIdx.x == 0)     // levels masked for the dense path only if that kernel saw the same pyramid
         s_skip = (red_skip && host_levels.h[0] > 0 && !host_levels_match(host_levels, level_hw, level_start, L)) ? 0u : red_skip;
-    __shared__ unsigned s_mask16;
+    __shared__ unsigned s_mask16, s_mask_rep;
     if (gv16 != nullptr && threadIdx.x == 32) {
         // which levels lie in the fp16 part is decided from the DEVICE pyramid: a level is fine if it ends at or before
         // side_start, coarse if it starts at or after it; a level that straddles the split cannot be served by either
-        // buffer (the caller planned with shapes that are not the device's) and traps
-        unsigned mk = 0;
+        // buffer (the caller planned with shapes that are not the device's) and traps.  Likewise for the replicated
+        // levels among the fp16 ones: those that start at or after rep_start.
+        unsigned mk = 0, mr = 0;
         for (int l = 0; l < L; ++l) {
             const long long a = level_start[l], e = a + level_hw[2 * l] * level_hw[2 * l + 1];
-            if (e <= side_start) mk |= 1u << l;
-            else if (a < side_start) __trap();
+            if (e <= side_start) {
+                mk |= 1u << l;
+                if (a >= rep_start) mr |= 1u << l;
+                else if (e > rep_start) __trap();
+            } else if (a < side_start) {
+                __trap();
+            }
         }
         s_mask16 = mk;
+        s_mask_rep = mr;
     }
     load_level_tab(level_hw, level_start, L, M * 32, tab);
     red_skip = s_skip;
-    if (gv16 != nullptr) gv16_mask = s_mask16;
+    unsigned rep_mask = 0;
+    if (gv16 != nullptr) { gv16_mask = s_mask16; rep_mask = s_mask_rep; }
+    const int S_rep = side_start - rep_start;
+    const int S16 = rep_start + rep_k * S_rep;                             // pixels of one map of gv16
     const float gv_sc = gv_amax ? gv16_scale(__ldg(gv_amax)) : 1.f;       // scale of the fp16 accumulators
     constexpr bool kGvFx = sizeof(TV) == 8;
     double fx_sc = 0.0;
@@ -234,6 +249,7 @@ msda_bwd_d32(const T *__restrict__ value, const int64_t *__restrict__ level_hw,
     if (b < 0) { live = false; b = 0; }           // row_map -1: unused row of a fixed-capacity list
     const int pix = M * 32;
     const int LP = L * P;
+    const long long rep_ofs = rep_mask ? (long long)((row / M) % rep_k) * S_rep * pix : 0;   // this pair row's copy
     const long long voff = ((long long)b * S * M + m) * 32 + sub * VEC;
     const float2 *locp = reinterpret_cast<const float2 *>(loc) + row * LP;
     const float *attp = attn + row * LP;
@@ -388,8 +404,8 @@ msda_bwd_d32(const T *__restrict__ value, const int64_t *__restrict__ level_hw,
                 if (q10 != 0.f) red_add_v4(gp + oy, q10 * gra[0], q10 * gra[1], q10 * gra[2], q10 * gra[3]);
                 if (q11 != 0.f) red_add_v4(gp + oy + ox, q11 * gra[0], q11 * gra[1], q11 * gra[2], q11 * gra[3]);
             } else if ((gv16_mask >> l) & 1u) {
-                // mixed mode, a fine level: scaled fp16 accumulation into the fine buffer (map stride side_start)
-                __half *gp = gv16 + (o00 - (long long)b * S_side * pix);
+                // mixed mode, a fine or replicated level: scaled fp16 accumulation into gv16 (map stride S16)
+                __half *gp = gv16 + (o00 - (long long)b * (S - S16) * pix + (((rep_mask >> l) & 1u) ? rep_ofs : 0));
                 auto red8 = [&](__half *p, float q) {
                     q *= gv_sc;
                     red_add_v4_f16x2(p, pack_f16x2(q * g[0], q * g[1]), pack_f16x2(q * g[2], q * g[3]),
@@ -740,9 +756,10 @@ static int launch_splat(const char *who, const float *loc, const float *attn, co
 
 struct MixedGv {               // scaled-fp16 / mixed accumulation of grad_value (see msda_bwd_d32)
     const unsigned *amax = nullptr;          // float bits of max|grad_out| (bevf_abs_max)
-    __half *gv16 = nullptr;                  // mixed mode: the fine levels' buffer
+    __half *gv16 = nullptr;                  // mixed mode: the fine and replicated levels' buffer
     unsigned mask = 0;
     int side_start = 0, S_side = 0;
+    int rep_start = 0, rep_k = 1;            // replicated levels: pixels [rep_start, side_start), rep_k copies
 };
 
 struct FxGv {                  // 64-bit fixed-point grad_value (deterministic mode)
@@ -800,7 +817,7 @@ static int launch_bwd(const char *who, const void *value, const int64_t *hw, con
                     msda_bwd_d32<T, TG, true, float, true><<<grid, kThreads, 0, st>>>(
                         (const T *)value, hw, ls, nullptr, nullptr, (const TG *)go, gv, gl, ga, row_map, S, M, Q, L, P,
                         (65536 + P - 1) / P, 1, rows, done_levels, hl, mixed->amax, mixed->gv16, mixed->mask,
-                        mixed->side_start, mixed->S_side, nullptr, 0, *fz);
+                        mixed->side_start, mixed->S_side, nullptr, 0, *fz, mixed->rep_start, mixed->rep_k);
                 else
                     return fail("%s: the fused prep needs a bf16 grad_out", who);
                 return check_launch(who);
@@ -808,7 +825,8 @@ static int launch_bwd(const char *who, const void *value, const int64_t *hw, con
             msda_bwd_d32<T, TG, true><<<grid, kThreads, 0, st>>>((const T *)value, hw, ls, loc, attn, (const TG *)go, gv, gl, ga,
                                                                row_map, S, M, Q, L, P, (65536 + P - 1) / P, 1, rows,
                                                                done_levels, hl, mixed->amax, mixed->gv16, mixed->mask, mixed->side_start,
-                                                               mixed->S_side);
+                                                               mixed->S_side, nullptr, 0, ScaFuse{}, mixed->rep_start,
+                                                               mixed->rep_k);
             return check_launch(who);
         } else {
             return fail("%s: mixed accumulation needs a bf16 value tensor", who);
@@ -1095,17 +1113,21 @@ static int rows_backward_mixed_impl(const char *who, const void *value, int valu
                                     const int64_t *level_start, const int32_t *level_hw_host, const float *loc,
                                     const float *attn, const void *grad_out, int grad_out_dtype,
                                     void *grad_value_fine_f16, float *grad_value_side, const uint32_t *amax_bits,
-                                    int num_f16_levels, int first_dense_level, float *grad_loc, float *grad_attn,
-                                    const int32_t *row_map, const int32_t *group_order, const int32_t *map_range,
-                                    int B, int S, int M, int D, int R, int L, int P, void *stream,
-                                    const ScaFuse *fz = nullptr) {
+                                    int num_f16_levels, int num_rep_levels, int replicas, int first_dense_level,
+                                    float *grad_loc, float *grad_attn, const int32_t *row_map,
+                                    const int32_t *group_order, const int32_t *map_range, int B, int S, int M, int D,
+                                    int R, int L, int P, void *stream, const ScaFuse *fz = nullptr) {
     if (!row_map && R > 0) return fail("%s: row_map is null", who);
-    if (!level_hw_host || !grad_value_fine_f16 || !grad_value_side || !amax_bits)
-        return fail("%s: null pointer argument", who);
     if (L <= 1 || L > kMaxLevels || num_f16_levels < 1 || num_f16_levels >= L)
         return fail("%s: num_f16_levels must be in [1, L - 1]", who);
-    if (map_range && (first_dense_level < num_f16_levels || first_dense_level >= L))
-        return fail("%s: first_dense_level must be in [num_f16_levels, L - 1]", who);
+    if (num_rep_levels < 0 || num_rep_levels > L - num_f16_levels || replicas < 1 || replicas > 64)
+        return fail("%s: num_rep_levels must be in [0, L - num_f16_levels] and replicas in [1, 64]", who);
+    const int num_side_from = num_f16_levels + num_rep_levels;       // first level of the fp32 side buffer
+    // (no side levels: grad_value_side is never touched and may be NULL)
+    if (!level_hw_host || !grad_value_fine_f16 || (!grad_value_side && num_side_from < L) || !amax_bits)
+        return fail("%s: null pointer argument", who);
+    if (map_range && (first_dense_level < num_side_from || first_dense_level >= L))
+        return fail("%s: first_dense_level must be in [num_f16_levels + num_rep_levels, L - 1]", who);
     if (value_dtype != BEVF_DTYPE_BF16 || D != 32) return fail("%s: needs a bf16 value tensor and head_dim 32", who);
     if (!aligned16(grad_value_fine_f16) || !aligned16(grad_value_side))
         return fail("%s: device pointers must be 16-byte aligned", who);
@@ -1123,8 +1145,14 @@ static int rows_backward_mixed_impl(const char *who, const void *value, int valu
     mx.amax = amax_bits;
     mx.gv16 = reinterpret_cast<__half *>(grad_value_fine_f16);
     mx.mask = (1u << num_f16_levels) - 1u;
-    mx.side_start = hl.start[num_f16_levels];
+    mx.rep_start = hl.start[num_f16_levels];
+    mx.side_start = num_side_from < L ? hl.start[num_side_from] : S;
+    // no side levels: nothing is written to the side buffer, the launch below only needs a non-null pointer
+    if (!grad_value_side) grad_value_side = reinterpret_cast<float *>(grad_value_fine_f16);
     mx.S_side = S - mx.side_start;
+    mx.rep_k = replicas;
+    if ((long long)(mx.rep_start + (long long)replicas * (mx.side_start - mx.rep_start)) * M * D >= (1ll << 31))
+        return fail("%s: one map of grad_value_fine_f16 exceeds 2^31 elements", who);
     cudaStream_t st = (cudaStream_t)stream;
     unsigned dense_levels = 0;                       // levels whose grad_value the dense kernel produced
     cudaEvent_t join = nullptr;
@@ -1179,7 +1207,7 @@ extern "C" int bevf_msda_rows_backward_mixed(const void *value, int value_dtype,
                                              int B, int S, int M, int D, int R, int L, int P, void *stream) {
     return rows_backward_mixed_impl("bevf_msda_rows_backward_mixed", value, value_dtype, level_hw, level_start,
                                     level_hw_host, loc, attn, grad_out, grad_out_dtype, grad_value_fine_f16,
-                                    grad_value_side, amax_bits, num_f16_levels, L, grad_loc, grad_attn, row_map,
+                                    grad_value_side, amax_bits, num_f16_levels, 0, 1, L, grad_loc, grad_attn, row_map,
                                     group_order, nullptr, B, S, M, D, R, L, P, stream);
 }
 
@@ -1194,9 +1222,26 @@ extern "C" int bevf_msda_rows_backward_mixed_dense(const void *value, int value_
     const char *who = "bevf_msda_rows_backward_mixed_dense";
     if (!map_range) return fail("%s: null pointer argument", who);
     return rows_backward_mixed_impl(who, value, value_dtype, level_hw, level_start, level_hw_host, loc, attn, grad_out,
-                                    grad_out_dtype, grad_value_fine_f16, grad_value_side, amax_bits, num_f16_levels,
-                                    first_dense_level, grad_loc, grad_attn, row_map, nullptr, map_range, B, S, M, D, R,
-                                    L, P, stream);
+                                    grad_out_dtype, grad_value_fine_f16, grad_value_side, amax_bits, num_f16_levels, 0,
+                                    1, first_dense_level, grad_loc, grad_attn, row_map, nullptr, map_range, B, S, M, D,
+                                    R, L, P, stream);
+}
+
+extern "C" int bevf_msda_rows_backward_replicated(const void *value, int value_dtype, const int64_t *level_hw,
+                                                  const int64_t *level_start, const int32_t *level_hw_host,
+                                                  const float *loc, const float *attn, const void *grad_out,
+                                                  int grad_out_dtype, void *grad_value_f16, float *grad_value_side,
+                                                  const uint32_t *amax_bits, int num_f16_levels, int num_rep_levels,
+                                                  int replicas, int first_dense_level, float *grad_loc,
+                                                  float *grad_attn, const int32_t *row_map,
+                                                  const int32_t *group_order, const int32_t *map_range, int B, int S,
+                                                  int M, int D, int R, int L, int P, void *stream) {
+    const char *who = "bevf_msda_rows_backward_replicated";
+    if (group_order && map_range) return fail("%s: group_order and map_range exclude each other", who);
+    return rows_backward_mixed_impl(who, value, value_dtype, level_hw, level_start, level_hw_host, loc, attn, grad_out,
+                                    grad_out_dtype, grad_value_f16, grad_value_side, amax_bits, num_f16_levels,
+                                    num_rep_levels, replicas, map_range ? first_dense_level : L, grad_loc, grad_attn,
+                                    row_map, group_order, map_range, B, S, M, D, R, L, P, stream);
 }
 
 // ---- SpatialCrossAttention's sampler with the sampling-point prep fused in (ScaFuse, msda_common.cuh) ----------
@@ -1247,6 +1292,28 @@ extern "C" int bevf_sca_rows_forward_fused(const void *value, int value_dtype, c
                              B, S, M, D, R, L, P, stream, &fz);
 }
 
+static int sca_rows_backward_fused_impl(
+    const char *who, const void *value, int value_dtype, const int64_t *level_hw, const int64_t *level_start,
+    const int32_t *level_hw_host, const float *raw, const float *stats, const float *coarse_loc,
+    const float *coarse_attn, int coarse_from, const float *ref_cam, const int32_t *pair_q, const int32_t *pair_cam,
+    const int32_t *pair_of, const void *grad_out, int grad_out_dtype, void *grad_value_f16, float *grad_value_side,
+    const uint32_t *amax_bits, int num_f16_levels, int num_rep_levels, int replicas, int first_dense_level,
+    float *grad_loc, float *grad_attn, void *d_raw, const int32_t *row_map, const int32_t *map_range, int B, int S,
+    int M, int D, int R, int L, int P, int bs, int Nq, int pairs, int Dz, int ncam, void *stream) {
+    if (R == 0) return 0;
+    ScaFuse fz;
+    if (int e = sca_fuse_args(who, raw, ref_cam, pair_q, pair_cam, pair_of, stats, coarse_loc, coarse_attn,
+                              coarse_from, M, D, R, L, P, bs, Nq, pairs, Dz, ncam, fz))
+        return e;
+    if (!pair_of) return fail("%s: null pointer argument", who);
+    if (!d_raw || !aligned16(d_raw)) return fail("%s: d_raw must be a 16-byte aligned bf16 buffer", who);
+    fz.d_raw = reinterpret_cast<bf16 *>(d_raw);
+    return rows_backward_mixed_impl(who, value, value_dtype, level_hw, level_start, level_hw_host, nullptr, nullptr,
+                                    grad_out, grad_out_dtype, grad_value_f16, grad_value_side, amax_bits,
+                                    num_f16_levels, num_rep_levels, replicas, map_range ? first_dense_level : L,
+                                    grad_loc, grad_attn, row_map, nullptr, map_range, B, S, M, D, R, L, P, stream, &fz);
+}
+
 extern "C" int bevf_sca_rows_backward_fused(const void *value, int value_dtype, const int64_t *level_hw,
                                             const int64_t *level_start, const int32_t *level_hw_host, const float *raw,
                                             const float *stats, const float *coarse_loc, const float *coarse_attn,
@@ -1257,19 +1324,28 @@ extern "C" int bevf_sca_rows_backward_fused(const void *value, int value_dtype, 
                                             float *grad_loc, float *grad_attn, void *d_raw, const int32_t *row_map,
                                             const int32_t *map_range, int B, int S, int M, int D, int R, int L, int P,
                                             int bs, int Nq, int pairs, int Dz, int ncam, void *stream) {
-    const char *who = "bevf_sca_rows_backward_fused";
-    if (R == 0) return 0;
-    ScaFuse fz;
-    if (int e = sca_fuse_args(who, raw, ref_cam, pair_q, pair_cam, pair_of, stats, coarse_loc, coarse_attn,
-                              coarse_from, M, D, R, L, P, bs, Nq, pairs, Dz, ncam, fz))
-        return e;
-    if (!pair_of) return fail("%s: null pointer argument", who);
-    if (!d_raw || !aligned16(d_raw)) return fail("%s: d_raw must be a 16-byte aligned bf16 buffer", who);
-    fz.d_raw = reinterpret_cast<bf16 *>(d_raw);
-    return rows_backward_mixed_impl(who, value, value_dtype, level_hw, level_start, level_hw_host, nullptr, nullptr,
-                                    grad_out, grad_out_dtype, grad_value_fine_f16, grad_value_side, amax_bits,
-                                    num_f16_levels, map_range ? first_dense_level : L, grad_loc, grad_attn, row_map,
-                                    nullptr, map_range, B, S, M, D, R, L, P, stream, &fz);
+    return sca_rows_backward_fused_impl("bevf_sca_rows_backward_fused", value, value_dtype, level_hw, level_start,
+                                        level_hw_host, raw, stats, coarse_loc, coarse_attn, coarse_from, ref_cam, pair_q,
+                                        pair_cam, pair_of, grad_out, grad_out_dtype, grad_value_fine_f16,
+                                        grad_value_side, amax_bits, num_f16_levels, 0, 1, first_dense_level, grad_loc,
+                                        grad_attn, d_raw, row_map, map_range, B, S, M, D, R, L, P, bs, Nq, pairs, Dz,
+                                        ncam, stream);
+}
+
+extern "C" int bevf_sca_rows_backward_fused_replicated(
+    const void *value, int value_dtype, const int64_t *level_hw, const int64_t *level_start,
+    const int32_t *level_hw_host, const float *raw, const float *stats, const float *coarse_loc,
+    const float *coarse_attn, int coarse_from, const float *ref_cam, const int32_t *pair_q, const int32_t *pair_cam,
+    const int32_t *pair_of, const void *grad_out, int grad_out_dtype, void *grad_value_f16, float *grad_value_side,
+    const uint32_t *amax_bits, int num_f16_levels, int num_rep_levels, int replicas, int first_dense_level,
+    float *grad_loc, float *grad_attn, void *d_raw, const int32_t *row_map, const int32_t *map_range, int B, int S,
+    int M, int D, int R, int L, int P, int bs, int Nq, int pairs, int Dz, int ncam, void *stream) {
+    return sca_rows_backward_fused_impl("bevf_sca_rows_backward_fused_replicated", value, value_dtype, level_hw,
+                                        level_start, level_hw_host, raw, stats, coarse_loc, coarse_attn, coarse_from,
+                                        ref_cam, pair_q, pair_cam, pair_of, grad_out, grad_out_dtype, grad_value_f16,
+                                        grad_value_side, amax_bits, num_f16_levels, num_rep_levels, replicas,
+                                        first_dense_level, grad_loc, grad_attn, d_raw, row_map, map_range, B, S, M, D,
+                                        R, L, P, bs, Nq, pairs, Dz, ncam, stream);
 }
 
 namespace bevf {

@@ -7,6 +7,7 @@ the current stream only; all arithmetic happens in ``libbevformer_b200.so``.
 """
 from __future__ import annotations
 
+import math
 import os
 import warnings
 
@@ -353,14 +354,45 @@ def dense_levels_for(rows_per_map: float, num_points: int, level_hw_host):
     return first
 
 
+def gv_replicas_for(rows_per_map: float, num_points: int, level_hw_host):
+    """{level: k} for the mixed backward's REPLICATED fp16 levels: those that gv_mode_for leaves in fp32 and
+    dense_levels_for does not take (at base: level 2, 164 contributions per pixel) accumulate in scaled fp16 into
+    k = ceil(contributions / BEVF_GV_MAXCONTRIB) copies, pair row r into copy r % k, so that each copy sums about as
+    many contributions as a fine level; the merge adds the copies in fp32.  Half the L2 reduction sectors of fp32 and
+    the colliding rows spread over k addresses.  Empty where gv_mode_for picks no mixed mode (BEVF_GV_ACC=fp32, TSA)."""
+    mode = gv_mode_for(rows_per_map, num_points, level_hw_host)
+    if not isinstance(mode, tuple):
+        return {}
+    _, shapes, nfine = mode
+    cap = float(os.environ.get("BEVF_GV_MAXCONTRIB", "64"))
+    kd = dense_levels_for(rows_per_map, num_points, shapes)
+    out = {}
+    for l in range(nfine, len(shapes) if kd is None else kd):
+        h, w = shapes[l]
+        out[l] = int(math.ceil(rows_per_map * num_points * 4.0 / (h * w) / cap))
+    return out
+
+
+def replica_plan(replicas, num_f16_levels):
+    """(num_rep_levels, k) the replicated backward takes from a gv_replicas_for result: its levels directly follow
+    the ``num_f16_levels`` fine ones and share one copy count, the largest; (0, 1) for none."""
+    if not replicas:
+        return 0, 1
+    levels = sorted(replicas)
+    if levels != list(range(num_f16_levels, num_f16_levels + len(levels))):
+        raise RuntimeError("replicated grad_value levels must directly follow the fp16 ones")
+    return len(levels), max(replicas.values())
+
+
 class LazyGradValue:
     """grad_value of a sampler backward still in accumulator form (scaled fp16 [+ fp32 side buffer]): ``materialize()``
-    runs the one conversion pass (bevf_gv16_unscale / bevf_gv_merge) on the CURRENT stream and returns the bf16
-    gradient.  Lets the consumer (plugin/linear.py's shared projections) do that pass off the critical path, exactly
-    where it converts an fp32 grad_value."""
+    runs the one conversion pass (bevf_gv16_unscale / bevf_gv_merge[_replicated]) on the CURRENT stream and returns
+    the bf16 gradient.  Lets the consumer (plugin/linear.py's shared projections) do that pass off the critical path,
+    exactly where it converts an fp32 grad_value.  ``rep`` = (S_fine, S_rep, k): ``fine`` holds k copies of the
+    S_rep replicated pixels after its S_fine fine ones."""
 
-    def __init__(self, shape, fine, side, amax):
-        self.shape, self.fine, self.side, self.amax = tuple(shape), fine, side, amax
+    def __init__(self, shape, fine, side, amax, rep=None):
+        self.shape, self.fine, self.side, self.amax, self.rep = tuple(shape), fine, side, amax, rep
         self.tensors = tuple(t for t in (fine, side, amax) if t is not None)
         self.device = fine.device
 
@@ -369,7 +401,11 @@ class LazyGradValue:
         gv = torch.empty(self.shape, device=self.device, dtype=torch.bfloat16)
         lib = _lib.load()
         with torch.cuda.device(self.device):
-            if self.side is None:
+            if self.rep is not None:
+                s_fine, s_rep, k = self.rep
+                st = lib.bevf_gv_merge_replicated(self.fine.data_ptr(), _ptr(self.side), self.amax.data_ptr(),
+                                                  gv.data_ptr(), nb, s, s_fine, s_rep, k, m * d, _stream_ptr(gv))
+            elif self.side is None:
                 st = lib.bevf_gv16_unscale(self.fine.data_ptr(), self.amax.data_ptr(), gv.data_ptr(), gv.numel(),
                                            _stream_ptr(gv))
             else:
@@ -496,13 +532,14 @@ def msda_rows_backward_f16acc(value, spatial_shapes, level_start_index, loc, att
 
 def msda_rows_backward_mixed(value, spatial_shapes, level_start_index, level_hw_host, num_f16_levels, loc, attn,
                              row_map, grad_output, group_order=None, lazy=False, map_range=None,
-                             first_dense_level=None):
+                             first_dense_level=None, replicas=None):
     """Row-list backward with MIXED accumulation (bevf_msda_rows_backward_mixed): the first ``num_f16_levels`` levels
     in scaled fp16, the others in fp32 into a side buffer that only spans their pixels; one merge pass produces the
     bf16 gradient.  ``level_hw_host``: [(h, w), ...] python ints that MUST equal the device spatial_shapes.
     ``map_range`` (B, 2) int32 for row lists grouped by value map (instead of ``group_order``): the levels
     [first_dense_level, L) (default: every side level) come from the dense tensor-core kernel where its plan covers
-    them (bevf_msda_rows_backward_mixed_dense)."""
+    them (bevf_msda_rows_backward_mixed_dense).  ``replicas`` (gv_replicas_for): the levels after the fine ones that
+    accumulate in scaled fp16 copies instead of fp32 (bevf_msda_rows_backward_replicated)."""
     import ctypes
     for t, n in ((value, "value"), (loc, "sampling_loc"), (attn, "attn_weight"), (row_map, "row_map"),
                  (grad_output, "grad_output")):
@@ -519,7 +556,9 @@ def msda_rows_backward_mixed(value, spatial_shapes, level_start_index, level_hw_
         if group_order is not None or map_range.numel() != 2 * NB or map_range.dtype != torch.int32:
             raise RuntimeError("mixed-accumulation backward: map_range must be (B, 2) int32, without group_order")
     ss, ls = _level_tensors(value, spatial_shapes, level_start_index)
+    nrep, k = replica_plan(replicas, num_f16_levels)
     s_fine = sum(int(h) * int(w) for h, w in level_hw_host[:num_f16_levels])
+    s_rep = sum(int(h) * int(w) for h, w in level_hw_host[num_f16_levels:num_f16_levels + nrep])
     grad_output = grad_output.contiguous()
     grad_loc = torch.empty(loc.shape, device=value.device, dtype=torch.float32)
     grad_attn = torch.empty(attn.shape, device=value.device, dtype=torch.float32)
@@ -527,13 +566,17 @@ def msda_rows_backward_mixed(value, spatial_shapes, level_start_index, level_hw_
     lib = _lib.load()
     with torch.cuda.device(value.device), _timed("msda_rows_backward", value.device, (R, L)):
         amax = abs_max_bits(grad_output)
-        fine = torch.zeros((NB, s_fine, M, D), device=value.device, dtype=torch.float16)
-        side = torch.zeros((NB, S - s_fine, M, D), device=value.device, dtype=torch.float32)
+        fine = torch.zeros((NB, s_fine + k * s_rep, M, D), device=value.device, dtype=torch.float16)
+        side = torch.zeros((NB, S - s_fine - s_rep, M, D), device=value.device, dtype=torch.float32)
         args = (value.data_ptr(), _DT[value.dtype], ss.data_ptr(), ls.data_ptr(), ctypes.addressof(hw), loc.data_ptr(),
-                attn.data_ptr(), grad_output.data_ptr(), _DT[grad_output.dtype], fine.data_ptr(), side.data_ptr(),
+                attn.data_ptr(), grad_output.data_ptr(), _DT[grad_output.dtype], fine.data_ptr(), _ptr(side),
                 amax.data_ptr(), int(num_f16_levels))
         tail = (grad_loc.data_ptr(), grad_attn.data_ptr(), row_map.data_ptr())
-        if map_range is None:
+        if nrep:
+            kd = num_f16_levels + nrep if first_dense_level is None else int(first_dense_level)
+            st = lib.bevf_msda_rows_backward_replicated(*args, nrep, k, kd, *tail, _ptr(group_order), _ptr(map_range),
+                                                        NB, S, M, D, R, L, P, _stream_ptr(value))
+        elif map_range is None:
             st = lib.bevf_msda_rows_backward_mixed(*args, *tail, _ptr(group_order), NB, S, M, D, R, L, P,
                                                    _stream_ptr(value))
         else:
@@ -541,7 +584,8 @@ def msda_rows_backward_mixed(value, spatial_shapes, level_start_index, level_hw_
             st = lib.bevf_msda_rows_backward_mixed_dense(*args, kd, *tail, map_range.data_ptr(), NB, S, M, D, R, L, P,
                                                          _stream_ptr(value))
         _lib.check(st, lib)
-    gv = LazyGradValue(value.shape, fine, side, amax)
+    gv = LazyGradValue(value.shape, fine, side if side.numel() else None, amax,
+                       (s_fine, s_rep, k) if nrep else None)
     return (gv if lazy else gv.materialize()), grad_loc, grad_attn
 
 
@@ -567,8 +611,9 @@ class SamplerRows(Function):
         out = msda_rows_forward(value, spatial_shapes, level_start_index, loc, attn, row_map)
         ctx.save_for_backward(value, loc, attn, row_map, spatial_shapes, level_start_index)
         ctx.group_order = group_order
-        # grad_value accumulated in scaled fp16 -- "f16": every level, ("mixed", level_hw_host, n): the first n levels
-        # -- (half the L2 reduction sectors of those levels): only where the caller asks for it
+        # grad_value accumulated in scaled fp16 -- "f16": every level, ("mixed", level_hw_host, n[, replicas]): the
+        # first n levels [and the replicated ones of gv_replicas_for] -- (half the L2 reduction sectors of those
+        # levels): only where the caller asks for it
         ctx.gv_mode = gv_mode if (gv_mode is not None and value.dtype == torch.bfloat16 and value.shape[-1] == 32) else None
         ctx.dense = dense if (dense is not None and not half and value.shape[-1] == 32) else None
         ctx.value_early = getattr(value, "_bevf_early", None)     # see plugin/linear.py::shared_input_projections
@@ -589,7 +634,8 @@ class SamplerRows(Function):
                 gv, gl, ga = msda_rows_backward_f16acc(value, ss, ls, loc, attn, row_map, grad_out, ctx.group_order,
                                                        lazy=True)
             else:
-                _, hw_host, nfine = ctx.gv_mode
+                hw_host, nfine = ctx.gv_mode[1:3]
+                reps = ctx.gv_mode[3] if len(ctx.gv_mode) > 3 else None     # gv_replicas_for, where the caller planned it
                 if sum(h * w for h, w in hw_host) != value.shape[1]:
                     # a stale host copy of the pyramid (it no longer adds up to S): plain fp32 accumulation instead
                     gv, gl, ga = msda_rows_backward(value, ss, ls, loc, attn, row_map, grad_out.contiguous(), None,
@@ -604,10 +650,10 @@ class SamplerRows(Function):
                     # levels [nfine, kd) fp32 reductions, [kd, L) on the tensor cores, both into the side buffer
                     gv, gl, ga = msda_rows_backward_mixed(value, ss, ls, hw_host, nfine, loc, attn, row_map, grad_out,
                                                           lazy=True, map_range=ctx.dense[1],
-                                                          first_dense_level=max(kd, nfine))
+                                                          first_dense_level=max(kd, nfine), replicas=reps)
                 else:
                     gv, gl, ga = msda_rows_backward_mixed(value, ss, ls, hw_host, nfine, loc, attn, row_map, grad_out,
-                                                          ctx.group_order, lazy=True)
+                                                          ctx.group_order, lazy=True, replicas=reps)
             if ctx.value_early is not None and ctx.value_early(gv):
                 return None, gl, ga, None, None, None, None, None, None      # the producer converts it off the critical path
             return gv.materialize(), gl, ga, None, None, None, None, None, None
@@ -704,12 +750,13 @@ def sca_rows_forward_fused(value, spatial_shapes, level_start_index, raw, ref_ca
 
 def sca_rows_backward_fused(value, spatial_shapes, level_start_index, level_hw_host, num_f16_levels, raw, stats,
                             ref_cam, pair_q, pair_cam, pair_of, row_map, grad_output, bs, nq, map_range=None,
-                            first_dense_level=None, coarse=None):
+                            first_dense_level=None, coarse=None, replicas=None):
     """Backward of sca_rows_forward_fused with msda_rows_backward_mixed's grad_value accumulation (``map_range``: the
     coarse levels from ``first_dense_level`` on through the dense tensor-core kernel, which reads the forward's
     ``coarse`` samples; without them those levels stay on the reduction path).  Returns (grad_value as a
     LazyGradValue, d_raw (bs*Nq, 768) bf16): the sampler finishes the d_raw rows of queries seen by one camera, the
-    finish kernel (bevf_sca_prep_backward_multi) the others from the sampler's grad_loc / grad_attn."""
+    finish kernel (bevf_sca_prep_backward_multi) the others from the sampler's grad_loc / grad_attn.  ``replicas``: as
+    for msda_rows_backward_mixed (bevf_sca_rows_backward_fused_replicated)."""
     import ctypes
     for t, n in ((value, "value"), (raw, "raw"), (stats, "stats"), (ref_cam, "ref_cam"), (pair_of, "pair_of"),
                  (row_map, "row_map"), (grad_output, "grad_output")):
@@ -722,7 +769,9 @@ def sca_rows_backward_fused(value, spatial_shapes, level_start_index, level_hw_h
     if not (1 <= num_f16_levels < L):
         raise RuntimeError("fused SCA backward: num_f16_levels does not fit the pyramid")
     ss, ls = _level_tensors(value, spatial_shapes, level_start_index)
+    nrep, k = replica_plan(replicas, num_f16_levels)
     s_fine = sum(int(h) * int(w) for h, w in level_hw_host[:num_f16_levels])
+    s_rep = sum(int(h) * int(w) for h, w in level_hw_host[num_f16_levels:num_f16_levels + nrep])
     grad_output = grad_output.contiguous()
     # scratch of the pair rows whose query more than one camera sees (only those rows are written)
     grad_loc = torch.empty((R, M, L, P, 2), device=value.device, dtype=torch.float32)
@@ -732,25 +781,27 @@ def sca_rows_backward_fused(value, spatial_shapes, level_start_index, level_hw_h
     lib = _lib.load()
     with torch.cuda.device(value.device), _timed("msda_rows_backward", value.device, (R, L)):
         amax = abs_max_bits(grad_output)
-        fine = torch.zeros((NB, s_fine, M, D), device=value.device, dtype=torch.float16)
-        side = torch.zeros((NB, S - s_fine, M, D), device=value.device, dtype=torch.float32)
-        kd = num_f16_levels if first_dense_level is None else int(first_dense_level)
-        st = lib.bevf_sca_rows_backward_fused(value.data_ptr(), _DT[value.dtype], ss.data_ptr(), ls.data_ptr(),
-                                              ctypes.addressof(hw), raw.data_ptr(), stats.data_ptr(),
-                                              _ptr(coarse and coarse[0]), _ptr(coarse and coarse[1]),
-                                              L if coarse is None else coarse[2], ref_cam.data_ptr(),
-                                              pair_q.data_ptr(), pair_cam.data_ptr(), pair_of.data_ptr(),
-                                              grad_output.data_ptr(), _DT[grad_output.dtype], fine.data_ptr(),
-                                              side.data_ptr(), amax.data_ptr(), int(num_f16_levels), kd,
-                                              grad_loc.data_ptr(), grad_attn.data_ptr(), d_raw.data_ptr(),
-                                              row_map.data_ptr(), _ptr(map_range), NB, S, M, D, R, L, P, bs, nq,
-                                              pair_q.numel(), ref_cam.shape[3], ref_cam.shape[0], _stream_ptr(value))
+        fine = torch.zeros((NB, s_fine + k * s_rep, M, D), device=value.device, dtype=torch.float16)
+        side = torch.zeros((NB, S - s_fine - s_rep, M, D), device=value.device, dtype=torch.float32)
+        kd = num_f16_levels + nrep if first_dense_level is None else int(first_dense_level)
+        head = (value.data_ptr(), _DT[value.dtype], ss.data_ptr(), ls.data_ptr(), ctypes.addressof(hw), raw.data_ptr(),
+                stats.data_ptr(), _ptr(coarse and coarse[0]), _ptr(coarse and coarse[1]),
+                L if coarse is None else coarse[2], ref_cam.data_ptr(), pair_q.data_ptr(), pair_cam.data_ptr(),
+                pair_of.data_ptr(), grad_output.data_ptr(), _DT[grad_output.dtype], fine.data_ptr(), _ptr(side),
+                amax.data_ptr(), int(num_f16_levels))
+        tail = (kd, grad_loc.data_ptr(), grad_attn.data_ptr(), d_raw.data_ptr(), row_map.data_ptr(), _ptr(map_range),
+                NB, S, M, D, R, L, P, bs, nq, pair_q.numel(), ref_cam.shape[3], ref_cam.shape[0], _stream_ptr(value))
+        if nrep:
+            st = lib.bevf_sca_rows_backward_fused_replicated(*head, nrep, k, *tail)
+        else:
+            st = lib.bevf_sca_rows_backward_fused(*head, *tail)
         _lib.check(st, lib)
     st = lib.bevf_sca_prep_backward_multi(raw.data_ptr(), grad_loc.data_ptr(), grad_attn.data_ptr(), pair_of.data_ptr(),
                                           ss.data_ptr(), d_raw.data_ptr(), BF16, bs, nq, pair_q.numel(), M, L, P,
                                           pair_of.shape[0], _stream_ptr(value))
     _lib.check(st, lib)
-    return LazyGradValue(value.shape, fine, side, amax), d_raw
+    return LazyGradValue(value.shape, fine, side if side.numel() else None, amax,
+                         (s_fine, s_rep, k) if nrep else None), d_raw
 
 
 def tsa_prep_forward(raw, ref2d, level_hw, B, Nq, M, L, P, interleave=False):

@@ -366,11 +366,11 @@ class _ScaHeadSamplerTC(Function):
     coefficient.  One autograd node, because the sampler backward produces d_raw in
     bf16: as a separate consumer of the fp32 ``raw`` it would be cast back to fp32 by autograd (and then to bf16
     again for the head's GEMMs).  ``fuse`` = (ref_cam, pair_q, pair_cam, pair_of, row_map, ss, lsi, bs, nq,
-    level_hw_host, num_f16_levels, map_range)."""
+    level_hw_host, num_f16_levels, map_range, replicas) -- replicas: ops.gv_replicas_for."""
 
     @staticmethod
     def forward(ctx, x, weight, bias, value, fuse):
-        ref_cam, pair_q, pair_cam, _pair_of, row_map, ss, lsi, bs, nq, hw_host, nfine, map_range = fuse
+        ref_cam, pair_q, pair_cam, _pair_of, row_map, ss, lsi, bs, nq, hw_host, nfine, map_range, _reps = fuse
         w = weight.to(x.dtype)
         xc = x.contiguous()
         raw = ops.linear_tc(xc, w, bias, None, False, torch.float32).reshape(-1, w.shape[0])
@@ -393,13 +393,14 @@ class _ScaHeadSamplerTC(Function):
     @once_differentiable
     def backward(ctx, grad_out):
         x, w, raw, stats, value = ctx.saved_tensors
-        ref_cam, pair_q, pair_cam, pair_of, row_map, ss, lsi, bs, nq, hw_host, nfine, map_range = ctx.fuse
+        ref_cam, pair_q, pair_cam, pair_of, row_map, ss, lsi, bs, nq, hw_host, nfine, map_range, reps = ctx.fuse
         coarse = ctx.coarse
         dense = coarse is not None and ops._lib.load().bevf_msda_get_dense_backward()
         gv, d_raw = ops.sca_rows_backward_fused(value, ss, lsi, hw_host, nfine, raw, stats, ref_cam, pair_q, pair_cam,
                                                 pair_of, row_map, grad_out, bs, nq,
                                                 map_range=map_range if dense else None,
-                                                first_dense_level=coarse[2] if dense else None, coarse=coarse)
+                                                first_dense_level=coarse[2] if dense else None, coarse=coarse,
+                                                replicas=reps)
         ctx.coarse = None
         gvalue = None
         if ctx.needs_input_grad[3] and not (ctx.value_early is not None and ctx.value_early(gv)):

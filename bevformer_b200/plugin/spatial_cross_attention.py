@@ -246,14 +246,18 @@ class SpatialCrossAttention(nn.Module):
         dense = None
         if level_hw_host is not None and plan.map_range is not None and len(level_hw_host) == l:
             dense = (level_hw_host, plan.map_range)
-        # grad_value of the fine pyramid levels accumulated in scaled fp16, the coarse ones in fp32 (ops.gv_mode_for)
+        # grad_value of the fine pyramid levels accumulated in scaled fp16, the coarse ones in fp32 (ops.gv_mode_for),
+        # those in between in replicated scaled-fp16 copies (ops.gv_replicas_for)
         gv_mode = None
         if level_hw_host is not None and len(level_hw_host) == l and v.dtype == torch.bfloat16:
-            gv_mode = ops.gv_mode_for(plan.row_map.numel() / max(1, bs * ncam), p, level_hw_host)
+            rows_per_map = plan.row_map.numel() / max(1, bs * ncam)
+            gv_mode = ops.gv_mode_for(rows_per_map, p, level_hw_host)
+            if isinstance(gv_mode, tuple):
+                gv_mode = gv_mode + (ops.gv_replicas_for(rows_per_map, p, level_hw_host),)
         if self._fused_prep(query, w, v, gv_mode, dense):
             # the sampling-point prep inside the sampler kernels: loc / attn never go through memory
             fuse = (plan.ref_cam, plan.pair_q, plan.pair_cam, plan.pair_of, plan.row_map, ss, lsi, bs, nq,
-                    gv_mode[1], gv_mode[2], plan.map_range)
+                    gv_mode[1], gv_mode[2], plan.map_range, gv_mode[3])
             out = sca_head_sampler(query, w, b, v, fuse)                                      # (bs*R, C)
         else:
             loc, attn = sca_sampling_head(query, w, b, plan.ref_cam, plan.pair_q, plan.pair_cam,

@@ -46,7 +46,7 @@
 extern "C" {
 #endif
 
-#define BEVF_ABI_VERSION 5
+#define BEVF_ABI_VERSION 6
 
 #if defined(__GNUC__)
 #define BEVF_API __attribute__((visibility("default")))
@@ -182,6 +182,18 @@ BEVF_API int bevf_msda_rows_backward_ordered(const void *value, int value_dtype,
  *                                             exactly bevf_msda_rows_backward_mixed.  Same outputs either way; the
  *                                             dense levels' coefficients are rounded to bf16 (2^-9 relative per term).
  *   bevf_gv_merge(fine, side, amax, out, B, S, S_fine, row_elems)   out (B, S, row_elems) bf16 from both
+ *   bevf_msda_rows_backward_replicated        bevf_msda_rows_backward_mixed (map_range NULL) or _mixed_dense (map_range
+ *                                             set, group_order NULL) with the num_rep_levels levels after the fine
+ *                                             ones (pixels [S_fine, S_fine + S_rep)) REPLICATED: accumulated in scaled
+ *                                             fp16 too, into `replicas` copies, pair row r adding into copy r % replicas
+ *                                             (each copy then sums about 1 / replicas of the contributions, as few as a
+ *                                             fine level's).  grad_value_f16 (B, S_fine + replicas * S_rep, M, D): the
+ *                                             fine pixels, then copy 0, 1, ... of the replicated ones; grad_value_side
+ *                                             (B, S - S_fine - S_rep, M, D) fp32 holds the levels after them (NULL if
+ *                                             none), first_dense_level in [num_f16_levels + num_rep_levels, L - 1]
+ *   bevf_gv_merge_replicated(f16, side, amax, out, B, S, S_fine, S_rep, replicas, row_elems)   out (B, S, row_elems)
+ *                                             bf16 from those two buffers, each replicated pixel the fp32 sum of its
+ *                                             copies; with S_rep = 0 it is bevf_gv_merge
  * All need a bf16 value tensor and head_dim 32 (fp16 value is an error); grad_loc / grad_attn are those of the fp32
  * path bit for bit.
  */
@@ -210,6 +222,18 @@ BEVF_API int bevf_msda_rows_backward_mixed_dense(const void *value, int value_dt
                                                  int B, int S, int M, int D, int R, int L, int P, void *stream);
 BEVF_API int bevf_gv_merge(const void *fine_f16, const float *side_f32, const uint32_t *amax_bits, void *out_bf16,
                            int B, int S, int S_fine, int row_elems, void *stream);
+BEVF_API int bevf_msda_rows_backward_replicated(const void *value, int value_dtype, const int64_t *level_hw,
+                                                const int64_t *level_start, const int32_t *level_hw_host,
+                                                const float *loc, const float *attn, const void *grad_out,
+                                                int grad_out_dtype, void *grad_value_f16, float *grad_value_side,
+                                                const uint32_t *amax_bits, int num_f16_levels, int num_rep_levels,
+                                                int replicas, int first_dense_level, float *grad_loc, float *grad_attn,
+                                                const int32_t *row_map, const int32_t *group_order,
+                                                const int32_t *map_range,
+                                                int B, int S, int M, int D, int R, int L, int P, void *stream);
+BEVF_API int bevf_gv_merge_replicated(const void *f16, const float *side_f32, const uint32_t *amax_bits,
+                                      void *out_bf16, int B, int S, int S_fine, int S_rep, int replicas,
+                                      int row_elems, void *stream);
 
 /*
  * DETERMINISTIC sampler backward: grad_value summed in 64-bit fixed point.  Integer addition is associative, so the
@@ -383,6 +407,16 @@ BEVF_API int bevf_sca_rows_backward_fused(const void *value, int value_dtype, co
                                           float *grad_loc, float *grad_attn, void *d_raw, const int32_t *row_map,
                                           const int32_t *map_range, int B, int S, int M, int D, int R, int L, int P,
                                           int bs, int Nq, int pairs, int Dz, int ncam, void *stream);
+/* bevf_sca_rows_backward_fused with bevf_msda_rows_backward_replicated's grad_value layout: num_rep_levels
+ * replicated fp16 levels after the fine ones, grad_value_f16 (B, S_fine + replicas * S_rep, 8, 32). */
+BEVF_API int bevf_sca_rows_backward_fused_replicated(
+    const void *value, int value_dtype, const int64_t *level_hw, const int64_t *level_start,
+    const int32_t *level_hw_host, const float *raw, const float *stats, const float *coarse_loc,
+    const float *coarse_attn, int coarse_from, const float *ref_cam, const int32_t *pair_q, const int32_t *pair_cam,
+    const int32_t *pair_of, const void *grad_out, int grad_out_dtype, void *grad_value_f16, float *grad_value_side,
+    const uint32_t *amax_bits, int num_f16_levels, int num_rep_levels, int replicas, int first_dense_level,
+    float *grad_loc, float *grad_attn, void *d_raw, const int32_t *row_map, const int32_t *map_range, int B, int S,
+    int M, int D, int R, int L, int P, int bs, int Nq, int pairs, int Dz, int ncam, void *stream);
 
 /* bevf_sca_prep_backward for the queries NOT seen by exactly one camera (0 cameras: zero rows; 2+: the sum over
  * their pair rows in camera order); the rows of one-camera queries are left as they are.  8 heads, L * P == 32,

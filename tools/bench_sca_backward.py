@@ -8,6 +8,9 @@ The SCA launch of the headline benchmark (the base rig's in-view pairs, 4 levels
                     bevf_msda_rows_backward_mixed_dense: levels [0, k) scaled fp16, levels [k, 4) on the tensor cores
   mixed_dense_k2_d3_{same,second}
                     levels 0-1 scaled fp16, level 2 fp32 reductions, level 3 on the tensor cores
+  replicated_d3_{same,second}
+                    bevf_msda_rows_backward_replicated: levels 0-1 scaled fp16, level 2 in the scaled-fp16 copies of
+                    ops.gv_replicas_for (3 at base), level 3 on the tensor cores
 Each timing is one op as the encoder issues it (scale source, zero-fill of the accumulators, the kernels), bracketed
 by CUDA events on the caller's stream (the second stream is joined into it); the bf16 conversion / merge pass is not
 included (it is the same pass for every mixed form).  The modes alternate in one process, ROUNDS x ITERS launches
@@ -58,10 +61,11 @@ def main():
     g = torch.Generator().manual_seed(1)
     gout = (torch.randn(loc.shape[0], 256, generator=g) * 0.1).to(dev, torch.bfloat16)
 
-    def mixed(k, dense, kd=None):
+    def mixed(k, dense, kd=None, replicas=None):
         def run():
             return ops.msda_rows_backward_mixed(vd, ss, lsi, levels, k, loc, attn, row_map, gout, lazy=True,
-                                                map_range=rng if dense else None, first_dense_level=kd)[0]
+                                                map_range=rng if dense else None, first_dense_level=kd,
+                                                replicas=replicas)[0]
         return run
 
     def dense_fp32():
@@ -73,6 +77,9 @@ def main():
         modes[f"mixed_dense_k{k}_second"] = (2, mixed(k, True))
     modes["mixed_dense_k2_d3_same"] = (1, mixed(2, True, 3))
     modes["mixed_dense_k2_d3_second"] = (2, mixed(2, True, 3))
+    reps = ops.gv_replicas_for(row_map.numel() / v.shape[0], loc.shape[3], levels)
+    modes["replicated_d3_same"] = (1, mixed(2, True, 3, reps))
+    modes["replicated_d3_second"] = (2, mixed(2, True, 3, reps))
     if args.modes:
         modes = {n: modes[n] for n in args.modes.split(",")}
 
